@@ -1,13 +1,17 @@
 """bench.py — denoised latent frames/sec of the SVI clip-denoising hot path (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload cfg2|cfg3|cfg4|cfg5|cfg1|tiny]
+                    [--dump-outputs DIR]
 
 Default workload cfg2 = BASELINE.json configs[1] (the configuration the metric is quoted on): a "step" is ONE
 flow-matching denoise step of the clip — two Wan-DiT forwards (classifier-free guidance) + the fused CFG/Euler update —
 on synthetic inputs (Wan2.1-T2V-1.3B, 81 frames x 480 x 832 -> latents [1,16,21,60,104], L = 32760 tokens, 512 text
 tokens, random-init weights).  value = 21 latent frames / (50 * seconds_per_step).  Timing: CUDA events on the launching
 stream, barrier + synchronize on both sides, max over ranks.  The working set of one step (2.8 GB of weights + ~1.5 GB
-of activations) is far larger than the 126 MB L2, so no explicit L2 flush is needed ("inputs larger than L2").
+of activations) is far larger than the 50 MB L2 of an H100, so no explicit L2 flush is needed ("inputs larger than L2").
+--dump-outputs DIR: after the timed steps, what the last timed step computed (the updated latents and, on one GPU, the
+conditional / unconditional velocities) goes to DIR/<name>.npy as float32; inputs are seeded, so two builds run with the
+same arguments can be compared output for output.
 
 Every step — timed (`value`, device-resident inputs) and end-to-end (`e2e`, pinned host buffers copied in and the updated
 latents copied out every step) — goes through the pipeline's own step function, SVIVideoPipeline.denoise_step, on one GPU
@@ -59,7 +63,7 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, d.get("bf16_tflops_sustained", d.get("bf16_tflops")), "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"
-    return {}, 1400.0, "fallback (B200_PROFILING.md sustained ~1.4 PFLOP/s)"
+    return {}, 989.0, "data sheet (H100 SXM dense BF16, 700 W; not measured)"
 
 
 def host_cpu():
@@ -107,6 +111,20 @@ class ClockSampler:
         pw = sorted(float(r[6]) for r in self.rows if len(r) > 6 and r[6].replace(".", "", 1).isdigit())
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx, "reasons": reasons, "samples": len(sm),
                 "power_w": pw[len(pw) // 2] if pw else None}
+
+
+def dump_outputs(dirname, arrays, budget_bytes=64 << 20):
+    """arrays: name -> tensor.  Each is written as DIR/<name>.npy in float32; one larger than its share of the budget is
+    replaced by a fixed, seeded sample of its elements (DIR/<name>_sample.npy, flattened, indices in increasing order)."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    share = budget_bytes // max(len(arrays), 1)
+    for name, t in arrays.items():
+        a = t.detach().float().cpu()
+        if a.numel() * 4 > share:
+            idx = torch.randperm(a.numel(), generator=torch.Generator().manual_seed(0))[:share // 4].sort().values
+            a, name = a.flatten()[idx], name + "_sample"
+        np.save(os.path.join(dirname, name + ".npy"), a.numpy())
 
 
 def build_model(cfg, device, lora_rank=0):
@@ -196,17 +214,10 @@ def run_reference_arm(args, wl_name, cfg, f, h, w, ctx_len, desc):
         return
     L = f * (h // 2) * (w // 2)
     times = []
-    budget_s = 170.0        # keep the whole arm within a few minutes on any host
-    t_start = time.perf_counter()
-    warm = args.warmup
-    for i in range(args.warmup + args.steps):
+    for i in range(args.warmup + args.steps):       # exactly --warmup untimed and --steps timed samples
         dt, cores, _, _ = cpu_block_baseline(cfg, L, ctx_len, (f, h // 2, w // 2))
-        if i == 0 and dt > 8.0:
-            warm = min(warm, 1)          # a >8 s sample: one untimed warm-up is all the budget allows
-        if i >= warm:
+        if i >= args.warmup:
             times.append(dt)
-        if len(times) >= args.steps or (times and time.perf_counter() - t_start > budget_s):
-            break
     t_blk = sum(times) / len(times)
     step_s = t_blk * cfg["num_layers"] * 2            # one denoise step = 2 forwards x num_layers blocks (+ negligible rest)
     value = f / (CLIP_STEPS * step_s)
@@ -265,7 +276,13 @@ def main():
     ap.add_argument("--no-vae", action="store_true", help="skip the clip-boundary VAE leg (decode 21->81 frames, encode 81 frames)")
     ap.add_argument("--no-sp-parity", action="store_true", help="N>1: skip the plan-vs-single-rank check before the timed run")
     ap.add_argument("--clips", type=int, default=10, help="cfg4: clips in the chain")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed to DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
+    if args.dump_outputs and (args.impl == "reference" or args.workload in ("cfg4", "cfg5")):
+        ap.error("--dump-outputs writes the outputs of the native denoise step: not available with --impl reference or "
+                 "--workload cfg4 / cfg5")
     if args.workload == "cfg4":
         from tools import clip_loop_bench
         return clip_loop_bench.main_from_bench(args)
@@ -360,8 +377,7 @@ def main():
 
     # the models are built: move every live Python object to the permanent generation so that a cyclic-GC pass triggered inside a
     # timed loop has (almost) nothing to traverse.  A full collection over the module trees is a host stall of tens of ms that the
-    # e2e leg (one synchronisation per step) cannot hide; whether that is what made one e2e step in three 22 ms longer
-    # (profiles/r02_f2_e2e_steps.txt) was not measured — this is hygiene, the per-step wall times stay on stderr
+    # e2e leg (one synchronisation per step) cannot hide; the per-step wall times stay on stderr
     import gc
     gc.collect()
     gc.freeze()
@@ -380,6 +396,11 @@ def main():
     e1.record()
     sync()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:     # before anything else runs a step on these buffers
+        outs = {"latents": lat}
+        if world == 1:
+            outs.update(velocity_cond=v_c, velocity_uncond=v_u)
+        dump_outputs(args.dump_outputs, outs)
     ms = e0.elapsed_time(e1)
     launches = eng.k.launches - launches0
     attn_ms = [a.elapsed_time(b) for a, b in eng.attn_events]
@@ -517,12 +538,8 @@ def main():
     if attn_ms:
         a_ms = sum(attn_ms) / len(attn_ms)
         ach = attn_flops / (a_ms * 1e-3) / 1e12
-        traffic = None   # DRAM bytes per launch from the committed ncu --set full capture (single-GPU shape only)
-        tpath = os.path.join(ROOT, "profiles", "attn_traffic.json")
-        if sp is None and args.workload == "cfg2" and os.path.exists(tpath):
-            traffic = json.load(open(tpath)).get("bytes_per_launch")
         roof = {"kernel": "attn_fwd_kernel (self-attention)", "bound": "tensor", "achieved": ach, "peak": peak,
-                "unit": "TFLOP/s", "frac": ach / peak, "traffic": traffic, "peak_source": peak_src,
+                "unit": "TFLOP/s", "frac": ach / peak, "peak_source": peak_src,
                 "launches_timed": len(attn_ms), "avg_ms": a_ms,
                 "share_of_step": sum(attn_ms) / ms}
     line = {"metric": METRIC, "value": value, "unit": "latent_frames/s",
@@ -532,7 +549,7 @@ def main():
                        "cfg_scale": CFG_SCALE, "clip_steps": CLIP_STEPS, "parallelism": plan,
                        "kv_exchange": None if sp is None or sp.sp_size == 1 else
                        ("NVLink peer push (copy engine) consumed by flag-gated attention" if sp._peer is not None else "NCCL all-gather"),
-                       "l2_policy": "inputs larger than L2 (weights + activations of a step >> 126 MB)",
+                       "l2_policy": "inputs larger than L2 (weights + activations of a step >> 50 MB)",
                        "numerics": "bf16 operands (two-term bf16 for the embedding / patch / head GEMMs), fp32 accumulate/residual/norm/softmax",
                        "lora_merged_layers": getattr(model, "lora_merged", 0)},
             "timed_mode": "eager launches + CUDA events around every self-attention launch (roofline leg)",

@@ -1,5 +1,5 @@
 /*
- * svi_b200.h — C ABI of the B200-native (sm_100a) kernel library for the SVI clip-denoising hot path.
+ * svi_b200.h — C ABI of the H100-native (sm_90a) kernel library for the SVI clip-denoising hot path.
  *
  * The reference (vita-epfl/Stable-Video-Infinity) has NO native boundary: its hot path is Python
  * (diffsynth) calling torch library kernels.  This header therefore DEFINES the boundary a maintainer
@@ -33,7 +33,7 @@ extern "C" {
 int svi_abi_version(void);
 /* Message of the last failing call made by this thread (never NULL). */
 const char* svi_last_error(void);
-/* Number of SMs of the current device (148 on B200); <0 on error. */
+/* Number of SMs of the current device (132 on H100 SXM); <0 on error. */
 int svi_sm_count(void);
 
 /*
@@ -55,7 +55,7 @@ typedef struct svi_gemm_epilogue {
   float* sumsq;          /* [M, sumsq_groups] f32, accumulated with atomicAdd (sumsq_parts == 0); or NULL */
   int32_t sumsq_groups;  /* number of column groups that are accumulated (columns beyond are skipped) */
   int32_t sumsq_group_cols; /* width of one group in columns; multiple of 32 */
-  /* ---- LayerNorm folded into the GEMM (M > 128 only; both sides optional, NULL = off) ------------------------------
+  /* ---- LayerNorm folded into the GEMM (both sides optional, NULL = off) ---------------------------------------------
    * Consumer: A = bf16(x[m,k] * g[k]) of the UN-normalised rows x and ln_stats[m] = (sum_k x, sum_k x^2) over ln_dim
    * columns; the epilogue reconstructs the product of the normalised, modulated rows:
    *     acc' = rstd_m * (acc - mean_m * ln_u[n]) ,  ln_u = W g   (then + bias: pass c = W t + b as `bias`)
@@ -72,7 +72,7 @@ typedef struct svi_gemm_epilogue {
 } svi_gemm_epilogue;
 
 /*
- * out = epilogue(A[M,K] @ W[N,K]^T), A and W bf16, fp32 accumulation on tcgen05 tensor cores (TMEM
+ * out = epilogue(A[M,K] @ W[N,K]^T), A and W bf16, fp32 accumulation on wgmma tensor cores (register
  * accumulators, TMA-fed 128B-swizzled operand tiles, persistent warp-specialised kernel).
  * Replaces every nn.Linear / F.linear on the path: wan_video_dit.py:227-229,242 (q,k,v,o),
  * :272-303 (cross-attn q,k,v,o,k_img,v_img), :334-335,372-373 (ffn.0/GELU/ffn.2 with gate+residual),
@@ -88,7 +88,7 @@ int svi_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, int32_
  * O: [Lq, ldo].  Any Lq, Lk >= 1 (ragged tails masked).  accumulate != 0: O += result
  * (used for the image branch of cross-attention, wan_video_dit.py:300-301).
  * workspace (optional, 16-byte aligned device memory of workspace_bytes, may be NULL / 0): lets the launch cut the
- * (head, Q-tile-pair) units of its last, partly filled wave of CTAs into K/V slices that are merged by a second
+ * (head, Q-tile) units of its last, partly filled wave of CTAs into K/V slices that are merged by a second
  * kernel (log-sum-exp merge), so all SMs stay busy; svi_attn_workspace_bytes() returns the size that allows every
  * plan.  The library never allocates.  Results are the same function of the inputs either way (fp32 merge).
  * Replaces flash_attention(), wan_video_dit.py:116-147 (the single attention entry point).
@@ -109,7 +109,7 @@ int svi_attn_fwd_qscale(const void* Q, int64_t ldq, const void* K, int64_t ldk, 
                         void* O, int64_t ldo, int32_t Lq, int32_t Lk, int32_t num_heads, float scale,
                         int32_t accumulate, const float* q_sumsq, int32_t q_ss_ld, int32_t q_ss_parts, int32_t q_dim,
                         float q_eps, void* workspace, size_t workspace_bytes, void* stream);
-/* The launch plan svi_attn_fwd uses (pure host function, no device needed): `units` = num_heads * ceil(Lq/256) equal
+/* The launch plan svi_attn_fwd uses (pure host function, no device needed): `units` = num_heads * ceil(Lq/128) equal
  * CTAs, kv_tiles = ceil(Lk/128), on `sms` SMs with a workspace of workspace_bytes -> units [0, n_full) run whole, the
  * rest are cut into `split` K/V slices each (split == 1: nothing is sliced). */
 void svi_attn_plan(int32_t units, int32_t kv_tiles, int32_t sms, size_t workspace_bytes, int32_t* n_full, int32_t* split);
@@ -255,7 +255,7 @@ int svi_axpby(const float* a, float alpha, const float* b, float beta, float* ou
 
 /*
  * One causal conv launch (CausalConv3d :33-52, Conv2d of Resample :82-174, time_conv, shortcut 1x1x1) as an
- * implicit GEMM on tcgen05.  Input: bf16 frame ring [ring_slots][in_H][in_W][C_in]; `slot[t*3 + a]` names the
+ * implicit GEMM on wgmma.  Input: bf16 frame ring [ring_slots][in_H][in_W][C_in]; `slot[t*3 + a]` names the
  * ring slot read by output frame t at temporal tap a (history frames stay in the ring — no pad/cat copies).
  * Input pixel = output pixel + (k_h - pad_h, k_w - pad_w); out-of-range pixels read as zero.
  * Weights: bf16 [w_rows, w_ld], row = output channel, column = ((a*kh + b)*kw + c)*ceil64(C_in) + channel.
@@ -283,10 +283,8 @@ typedef struct svi_conv_desc {
    * front of the second CausalConv3d of a ResidualBlock and between blocks (wan_video_vae.py:55-70, 206-210). */
   void* next_ring; int64_t next_frame_stride; int32_t next_ld; int32_t next_slot[4];
   const float* next_gamma; int32_t next_silu; int32_t write_f32;
-  /* Kernel choice (same results up to accumulation order).  1: one CTA per 128-pixel patch, one input box per tap.
-   * 2: CTA pairs (tcgen05 cta_group::2) on two image rows x 128 pixels; the input row window is loaded once per
-   * (k_t, k_h, 64-channel chunk) and the k_w taps read it at shifted row offsets, the weight tile is split between the
-   * two CTAs — needs k_w == 3 and pad_w == 1.  0: 2 where it applies and W >= 192, else 1. */
+  /* Kept for ABI compatibility only: 0, 1 or 2, and 2 is still refused unless k_w == 3 and pad_w == 1 so that existing
+   * callers see the same validation.  It selects nothing: every accepted value runs the same implicit-GEMM kernel. */
   int32_t variant;
 } svi_conv_desc;
 int svi_conv3d_causal(const svi_conv_desc* d, void* stream);

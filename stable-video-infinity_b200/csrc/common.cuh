@@ -1,6 +1,5 @@
-// Shared device/host helpers for the sm_100a kernels of the SVI clip-denoising hot path.
-// Everything here is inline PTX for Blackwell: mbarrier, TMA (cp.async.bulk.tensor), tcgen05
-// (TMEM alloc / mma / ld / st / commit) and the shared-memory / instruction descriptor encoders.
+// Shared device/host helpers for the sm_90a kernels of the SVI clip-denoising hot path: inline PTX for mbarrier and TMA
+// (cp.async.bulk.tensor), register redistribution, and the math helpers of the epilogues.  wgmma lives in wgmma.cuh.
 #pragma once
 
 #include <cuda.h>
@@ -55,274 +54,16 @@ int sm_count();
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return (uint32_t)__cvta_generic_to_shared(p);
 }
-__device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n"
-      ".reg .pred P;\n"
-      "elect.sync _|P, 0xffffffff;\n"
-      "selp.u32 %0, 1, 0, P;\n"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
 
 // ---------------------------------------------------------------------------------------------
-// mbarrier
+// mbarrier and TMA (32-bit shared-memory addresses: no generic 64-bit pointer arithmetic in the hot warps)
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
 __device__ __forceinline__ void fence_mbar_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)),
-               "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// Bounded spin: a protocol bug must trap (visible error) instead of hanging the GPU.
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 26)) {
-      printf("svi: mbarrier timeout block(%d,%d) thread %d bar %p parity %u\n", blockIdx.x,
-             blockIdx.y, threadIdx.x, (void*)bar, parity);
-      __trap();
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// TMA
-// ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory");
 }
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m, uint64_t* bar,
-                                            int c_inner, int c_outer) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(m), "r"(smem_u32(bar)), "r"(c_inner), "r"(c_outer)
-      : "memory");
-}
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src,
-                                             int c_inner, int c_outer) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(m),
-               "r"(smem_u32(smem_src)), "r"(c_inner), "r"(c_outer)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() {
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-}
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-template <int N>
-__device__ __forceinline__ void tma_store_wait() {
-  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
-}
-// make generic-proxy smem writes visible to the async proxy (TMA store / tcgen05.mma operand reads)
-__device__ __forceinline__ void fence_proxy_async_smem() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-
-// ---------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// all previously issued tcgen05.mma of this thread arrive on `bar` when complete
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-__device__ __forceinline__ void tc_mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]
-__device__ __forceinline__ void tc_mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-
-// ---- uniform-issue variants -------------------------------------------------------------------------------
-// The whole MMA warp executes these (no divergent `if (lane == 0)` around them): every operand is then
-// warp-uniform and ptxas keeps the descriptor arithmetic in uniform registers instead of building each
-// descriptor in vector registers and moving it over with R2UR (+ a compiler-inserted ELECT) per MMA, which cost
-// ~130 issue cycles per tcgen05.mma and made the single issuing thread the bottleneck (profiles/README.md).
-// The issuing lane is chosen by elect.sync inside each wrapper (deterministic for a full-warp mask, so every
-// mma / commit of the kernel comes from the same thread, as tcgen05.commit requires); `lead` is unused.
-__host__ __device__ __forceinline__ uint32_t smem_desc_lo(uint32_t smem_addr, uint32_t lbo_bytes) {
-  return ((smem_addr >> 4) & 0x3FFFu) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
-}
-__host__ __device__ constexpr uint32_t smem_desc_hi(uint32_t sbo_bytes, uint32_t layout_type) {
-  return ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 14) | ((layout_type & 7u) << 29);
-}
-__device__ __forceinline__ void tc_mma_ss_p(uint32_t lead, uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi,
-                                            uint32_t b_lo, uint32_t b_hi, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, q;\n"
-      ".reg .b64 da, db;\n"
-      "setp.ne.b32 p, %6, 0;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "mov.b64 da, {%1, %2};\n"
-      "mov.b64 db, {%3, %4};\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-  (void)lead;
-}
-__device__ __forceinline__ void tc_mma_ts_p(uint32_t lead, uint32_t d_tmem, uint32_t a_tmem, uint32_t b_lo,
-                                            uint32_t b_hi, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, q;\n"
-      ".reg .b64 db;\n"
-      "setp.ne.b32 p, %5, 0;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "mov.b64 db, {%2, %3};\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], db, %4, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-  (void)lead;
-}
-__device__ __forceinline__ void tc_commit_p(uint32_t lead, uint64_t* bar) {
-  asm volatile(
-      "{\n"
-      ".reg .pred q;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n"
-      "}\n" ::"r"(smem_u32(bar))
-      : "memory");
-  (void)lead;
-}
-
-// ---- batched issue: four consecutive K-steps (K = 64 bf16 = one 128-byte swizzle row) in ONE asm block ------
-// One elect.sync and one descriptor pair per batch; the per-step descriptor advance (+32 B = +2 in the 16-byte
-// start-address field) is plain 32-bit adds, so a 128x{64..256}x64 tile costs ~20 SASS instructions instead of
-// ~60.  The first MMA uses `acc_first` as the accumulate flag, the other three always accumulate.
-__device__ __forceinline__ void tc_mma_ss_k4(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo,
-                                             uint32_t b_hi, uint32_t idesc, uint32_t acc_first) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, q, t;\n"
-      ".reg .b64 da, db;\n"
-      ".reg .b32 a1, b1;\n"
-      "setp.ne.b32 p, %6, 0;\n"
-      "setp.eq.b32 t, 0, 0;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "mov.b64 da, {%1, %2};\n"
-      "mov.b64 db, {%3, %4};\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n"
-      "add.u32 a1, %1, 2;\n"
-      "add.u32 b1, %3, 2;\n"
-      "mov.b64 da, {a1, %2};\n"
-      "mov.b64 db, {b1, %4};\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, t;\n"
-      "add.u32 a1, %1, 4;\n"
-      "add.u32 b1, %3, 4;\n"
-      "mov.b64 da, {a1, %2};\n"
-      "mov.b64 db, {b1, %4};\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, t;\n"
-      "add.u32 a1, %1, 6;\n"
-      "add.u32 b1, %3, 6;\n"
-      "mov.b64 da, {a1, %2};\n"
-      "mov.b64 db, {b1, %4};\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, t;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(acc_first)
-      : "memory");
-}
-// A operand (P, bf16) in TMEM: +8 columns per K-step; B = MN-major V tile: +2048 B (16 rows x 128 B) per K-step
-__device__ __forceinline__ void tc_mma_ts_k4(uint32_t d_tmem, uint32_t a_tmem, uint32_t b_lo, uint32_t b_hi,
-                                             uint32_t idesc, uint32_t acc_first) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, q, t;\n"
-      ".reg .b64 db;\n"
-      ".reg .b32 a1, b1;\n"
-      "setp.ne.b32 p, %5, 0;\n"
-      "setp.eq.b32 t, 0, 0;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "mov.b64 db, {%2, %3};\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], db, %4, p;\n"
-      "add.u32 a1, %1, 8;\n"
-      "add.u32 b1, %2, 128;\n"
-      "mov.b64 db, {b1, %3};\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [a1], db, %4, t;\n"
-      "add.u32 a1, %1, 16;\n"
-      "add.u32 b1, %2, 256;\n"
-      "mov.b64 db, {b1, %3};\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [a1], db, %4, t;\n"
-      "add.u32 a1, %1, 24;\n"
-      "add.u32 b1, %2, 384;\n"
-      "mov.b64 db, {b1, %3};\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [a1], db, %4, t;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(acc_first)
-      : "memory");
-}
-
-// ---- 32-bit shared-address forms (no generic 64-bit pointer arithmetic in the hot warps) -----------------
 __device__ __forceinline__ void mbar_init_a(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
 }
@@ -346,11 +87,8 @@ __device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
         : "r"(bar), "r"(parity)
         : "memory");
     if (ok) break;
-    if (++spins > (1u << 26)) {
-      printf("svi: mbarrier timeout block(%d,%d) thread %d bar 0x%x parity %u\n", blockIdx.x, blockIdx.y,
-             threadIdx.x, bar, parity);
-      __trap();
-    }
+    // no printf here: a function call inside a wgmma pipeline makes ptxas serialise every wgmma of the kernel
+    if (++spins > (1u << 26)) __trap();
   }
 }
 __device__ __forceinline__ void tma_load_2d_a(uint32_t smem_dst, const CUtensorMap* m, uint32_t bar, int c_inner,
@@ -361,91 +99,11 @@ __device__ __forceinline__ void tma_load_2d_a(uint32_t smem_dst, const CUtensorM
       "l"(m), "r"(bar), "r"(c_inner), "r"(c_outer)
       : "memory");
 }
-__device__ __forceinline__ void tc_commit_a(uint32_t bar) {
-  asm volatile(
-      "{\n"
-      ".reg .pred q;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n"
-      "}\n" ::"r"(bar)
-      : "memory");
-}
-
-// 32 lanes x 32 consecutive 32-bit columns: thread i of the warp gets lane (base+i), cols [c, c+32)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-      "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]),
-      "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]),
-      "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
-// ---------------------------------------------------------------------------------------------
-// descriptors (bit layouts: cute/arch/mma_sm100_desc.hpp UMMA::SmemDescriptor / InstrDescriptor)
-// ---------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor. Byte offsets are encoded >> 4. version=1 (sm_100), base_offset 0.
-// layout_type: 0 none, 2 = 128B swizzle, 4 = 64B, 6 = 32B.
-__host__ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                            uint32_t sbo_bytes,
-                                                            uint32_t layout_type) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // version
-  d |= (uint64_t)(layout_type & 7) << 61;
-  return d;
-}
-// kind::f16 instruction descriptor: bf16 x bf16 -> fp32. a_major/b_major: 0 = K-major, 1 = MN-major.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_major,
-                                                       uint32_t b_major) {
-  return (1u << 4)      // c_format = F32
-         | (1u << 7)    // a_format = BF16
-         | (1u << 10)   // b_format = BF16
-         | (a_major << 15) | (b_major << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
+// Register redistribution between the warpgroups of a warp-specialised CTA (producer warpgroup gives, consumers take).
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);

@@ -103,7 +103,7 @@ layernorm_modulate_kernel(const float* __restrict__ x, int D, float eps, const f
 
 // Warp-per-row variant for D <= 2048 (the 1.3B model, D = 1536): no block barriers, the whole row is fetched with up
 // to 16 independent 16-byte loads per lane before anything is reduced (memory-level parallelism is what an HBM-bound
-// 6 KB-per-row kernel needs; the block-per-row version above reached only ~2.7 TB/s, profiles/README.md).
+// 6 KB-per-row kernel needs, and the block-per-row version above waits at its barriers with few loads in flight).
 constexpr int LNW_WARPS = 8;
 constexpr int LNW_MAX_VEC = 16;  // float4 per lane -> D <= 2048
 
@@ -190,7 +190,7 @@ rmsnorm_rope_kernel(__nv_bfloat16* __restrict__ t, long long ldt, int M, int D, 
     const int grp = cc >= D ? 1 : 0;
     const int c0 = cc - grp * D;                     // column inside the group
     // this thread's 8 values and weights first: the loads below them in program order would otherwise wait behind the
-    // partial-sum loads and the shuffles (two serialized memory latencies per thread: 101 -> 131 us at L = 32760)
+    // partial-sum loads and the shuffles (two serialized memory latencies per thread)
     uint4* ptr = reinterpret_cast<uint4*>(t + (long long)m * ldt + cc);
     const uint4 raw = *ptr;
     const float* wg = grp ? w2 : w;
@@ -409,8 +409,8 @@ __global__ void fold_combine_kernel(const float* __restrict__ o4, int N, const f
 
 inline int grid_for(long long n, int block) {
   long long g = (n + block - 1) / block;
-  const long long cap = 148LL * 16;
-  if (g > cap) g = cap;
+  const long long cap = 16LL * sm_count();   // grid-stride loops: 16 blocks per SM
+  if (cap > 0 && g > cap) g = cap;
   if (g < 1) g = 1;
   return (int)g;
 }

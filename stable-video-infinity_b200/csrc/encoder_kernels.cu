@@ -1,7 +1,7 @@
 // Kernels of the two conditioning encoders that run once per clip (umT5 text encoder, CLIP ViT image encoder):
 // token-embedding gather, T5 RMS norm, fp32-output LayerNorm, gated-activation product and a small-sequence attention
 // with arbitrary head width, additive relative-position bias and key mask.  The projections and MLPs of both encoders
-// run on svi_gemm_bf16 (tcgen05); what is here is HBM/latency-bound glue and the 512- / 257-token attention
+// run on svi_gemm_bf16 (wgmma); what is here is HBM/latency-bound glue and the 512- / 257-token attention
 // (0.2 % of the encoders' FLOPs), written as plain fp32 SIMT code.
 //
 // Replaces: reference diffsynth/models/wan_video_text_encoder.py (T5LayerNorm :22-35, T5Attention :55-89 incl. the
@@ -240,7 +240,8 @@ extern "C" int svi_mul_bf16(const void* a, const void* b, void* out, int64_t n, 
   using namespace svi;
   SVI_REQUIRE(a && b && out && n > 0 && n % 2 == 0, "svi_mul_bf16: n must be a positive even number");
   long long blocks = (n / 2 + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  const int cap = 16 * sm_count();   // grid-stride loop: 16 blocks per SM
+  if (cap > 0 && blocks > cap) blocks = cap;
   enc::mul_bf16_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const __nv_bfloat162*>(a), reinterpret_cast<const __nv_bfloat162*>(b),
       reinterpret_cast<__nv_bfloat162*>(out), n / 2);

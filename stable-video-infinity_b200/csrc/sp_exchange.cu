@@ -8,7 +8,7 @@
 // rank.  After a rank has produced its own rows (K|V GEMM + RMSNorm/RoPE epilogue kernels) it PUSHES them into the
 // same rows of every peer's buffer with copy-engine peer copies on a side stream, each followed by a 4-byte copy
 // of the layer's epoch number into the peer's flag word (same stream, so it lands after the rows; no SM is
-// involved, so the push can never wait for an SM that a spinning attention CTA holds).  The consumer is the attention kernel itself (attn_tcgen05.cu): its TMA producer warp
+// involved, so the push can never wait for an SM that a spinning attention CTA holds).  The consumer is the attention kernel itself (attn_wgmma.cu): its TMA producer warp
 // starts on the rank's own rows and polls a chunk's flag (ld.acquire.sys) only when the K/V stream reaches rows
 // owned by another rank, so the transfer overlaps the attention math tile by tile and no SM time is spent copying.
 #include <string.h>

@@ -174,8 +174,8 @@ softmax_rows_kernel(const float* __restrict__ s, int N, long long lds, float sca
 
 inline int grid_for(long long n, int block) {
   long long g = (n + block - 1) / block;
-  const long long cap = 148LL * 16;
-  if (g > cap) g = cap;
+  const long long cap = 16LL * sm_count();   // grid-stride loops: 16 blocks per SM
+  if (cap > 0 && g > cap) g = cap;
   if (g < 1) g = 1;
   return (int)g;
 }

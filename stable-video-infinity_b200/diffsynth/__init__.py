@@ -1,4 +1,4 @@
-"""B200-native drop-in for the reference's ``diffsynth`` package — hot path only.
+"""H100-native (sm_90a) drop-in for the reference's ``diffsynth`` package — hot path only.
 
 Exports the names ``test_svi.py`` imports (reference ``test_svi.py:2``):
 ``ModelManager``, ``save_video``, ``SVIVideoPipeline`` (+ ``WanVideoPipeline``).

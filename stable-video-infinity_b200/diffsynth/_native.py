@@ -1,6 +1,6 @@
 """ctypes binding of the C-ABI kernel library ``libsvi_b200.so`` (declared in ``include/svi_b200.h``).
 
-This is the only door between the Python host code and the hand-written sm_100a kernels.  There is no
+This is the only door between the Python host code and the hand-written sm_90a kernels.  There is no
 fallback: if the shared library is missing or a call fails, a ``RuntimeError`` is raised.
 """
 import ctypes
@@ -125,10 +125,10 @@ def load():
 
 
 def require_cuda(device, what):
-    """Every engine calls this first: the kernels exist for sm_100a only, so anything but a CUDA device is an error (there is
+    """Every engine calls this first: the kernels exist for sm_90a only, so anything but a CUDA device is an error (there is
     no CPU path), and the library must be loadable."""
     if torch.device(device).type != "cuda":
-        raise RuntimeError(f"svi_b200: {what} runs only on a CUDA device (sm_100a kernels; no CPU fallback)")
+        raise RuntimeError(f"svi_b200: {what} runs only on a CUDA device (sm_90a kernels; no CPU fallback)")
     load()
 
 
@@ -165,7 +165,7 @@ def sm_count():
 def gemm(a, w, out, bias=None, act=ACT_NONE, gate=None, residual=None, sumsq=None, sumsq_group_cols=0, ln=None, emit=None):
     """out = epilogue(a[M,K] @ w[N,K]^T); a, w bf16; out f32 or bf16 (may be a column slice view).
     ln = (stats f32 [M,2], u f32 [N], dim, eps): LayerNorm folded into the GEMM (consumer side, svi_gemm_epilogue);
-    emit = (a_next bf16 [M,N], g_next f32 [N], row_stats f32 [M,2]): producer side.  Both need M > 128."""
+    emit = (a_next bf16 [M,N], g_next f32 [N], row_stats f32 [M,2]): producer side."""
     lda, ldw, ldo = _rowmajor(a, "a"), _rowmajor(w, "w"), _rowmajor(out, "out")
     M, K = a.shape
     N = w.shape[0]
@@ -196,9 +196,6 @@ def gemm(a, w, out, bias=None, act=ACT_NONE, gate=None, residual=None, sumsq=Non
             if not sumsq.is_contiguous() or sumsq.shape[2] * 128 != sumsq_group_cols:
                 raise RuntimeError("svi_b200.gemm: partial sumsq must be contiguous [M, groups, sumsq_group_cols / 128]")
             ep.sumsq_parts = sumsq.shape[2]
-    if ln is not None or emit is not None:
-        if M <= 128:
-            raise RuntimeError("svi_b200.gemm: the LayerNorm fold runs in the CTA-pair kernel (M > 128)")
     if ln is not None:
         stats, u, dim, eps = ln
         if tuple(stats.shape) != (M, 2) or not stats.is_contiguous() or u.numel() != N:

@@ -233,7 +233,7 @@ def init_sp_groups(world=None, rank=None, cfg_parallel=True):
 
 def get_sp_group():
     """The process-wide plan behind `use_usp=True` (reference: xfuser's get_sp_group(), svi_video.py:266-273).  Default =
-    the measured plan: CFG-parallel x sequence-parallel for an even world size (N=2: cfg2 x sp1, N=8: cfg2 x sp4);
+    CFG-parallel x sequence-parallel for an even world size (N=2: cfg2 x sp1, N=8: cfg2 x sp4);
     SVI_SP_PLAN=sp splits only the token axis (sp = N), like the reference."""
     if _GROUP is None:
         if not dist.is_initialized():

@@ -1,6 +1,6 @@
 """Static LoRA merge  W += alpha * (B @ A)  at load time (reference diffsynth/models/lora.py:200-267).
 
-Key matching is host logic; the merge itself runs on the native tcgen05 GEMM (B as the row operand, A^T as the
+Key matching is host logic; the merge itself runs on the native wgmma GEMM (B as the row operand, A^T as the
 weight operand, alpha as the per-column gate and W as the fp32 residual), i.e. LoRA is folded through the same
 GEMM epilogue the north star names.  Result: W' = round_to_param_dtype(W + alpha * B A) with fp32 accumulation.
 """

@@ -1,9 +1,9 @@
-"""Wan DiT — host side of the B200-native hot path.
+"""Wan DiT — host side of the H100-native hot path.
 
 Same module/parameter names as the reference (``diffsynth/models/wan_video_dit.py``: ``WanModel`` :407-567,
 ``DiTBlock`` :321-374, ``SelfAttention`` :210-242, ``CrossAttention`` :245-303, ``Head`` :392-404,
 ``RMSNorm`` :186-197) so that Wan checkpoints and SVI LoRA keys load unchanged, but the nn.Modules are only
-PARAMETER CONTAINERS: all arithmetic runs in ``WanDiTEngine`` which drives the hand-written sm_100a kernels
+PARAMETER CONTAINERS: all arithmetic runs in ``WanDiTEngine`` which drives the hand-written sm_90a kernels
 of ``libsvi_b200.so`` through ``diffsynth._native`` (C ABI, ``include/svi_b200.h``).  There is no torch
 compute fallback: without a CUDA device + the built library every forward raises.
 
@@ -335,11 +335,10 @@ class WanDiTEngine:
         import os
         self.use_graphs = os.environ.get("SVI_CUDA_GRAPHS", "1") != "0"
         # SVI_LN_FOLD=1: LayerNorm + modulate folded into the GEMMs around it (no LayerNorm launch inside the block stack;
-        # forwards with more than 128 token rows per rank, no audio branch).  Built, parity-neutral (cfg-1: 0.961 either way)
-        # and MEASURED at the bench shape (profiles/r02_c4_perf.log, r02_step_breakdown_c4_*.txt): the three 51-58 us LayerNorm
-        # passes per block go away, but the consumer epilogues cost +28 us (ffn.0), +13 us (qkv / cross-q) and every producer
-        # +28 us (a further 100 MB bf16 write in an HBM-bound epilogue): 497.3 ms per step with the fold, 493.7 ms without.
-        # The faster path is the default; the fold stays selectable (and tested) as a design point.
+        # no audio branch).  The LayerNorm passes go away, but the consumer epilogues do more work and every producer writes
+        # a further bf16 copy of its output.  On an H100 (400 W power limit, bench shape, two alternating runs each) the step
+        # took 1733 / 1740 ms with the fold and 1734 / 1737 ms without: no measurable gain, so the plain path stays the
+        # default and the fold stays selectable (and tested) as a design point.
         self.use_fold = os.environ.get("SVI_LN_FOLD", "0") == "1"
         self._fold_static = None
         self.attn_events = None  # bench.py: list collecting (start, end) events around self-attention launches
@@ -767,7 +766,7 @@ class WanDiTEngine:
             cond_l = cond if sp is None else cond[sp.row_offset: sp.row_offset + Ll]
         nl = len(self.blocks)
         fold = None
-        if self.use_fold and ts.fold is not None and Ll > 128 and audio is None:
+        if self.use_fold and ts.fold is not None and audio is None:
             u2, c2 = self._fold_consts()
             fold = _FoldRun(ts.fold, u2, c2, self._buf("ln_stats", (nl, 3, Ll, 2), torch.float32))
             self.k.zero_(fold.stats)

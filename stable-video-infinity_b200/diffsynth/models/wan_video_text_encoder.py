@@ -4,7 +4,7 @@ Same module / parameter names as the reference (``diffsynth/models/wan_video_tex
 :209-255, ``T5SelfAttention`` :113-144, ``T5Attention`` :38-89, ``T5FeedForward`` :92-110, ``T5LayerNorm`` :22-35,
 ``T5RelativeEmbedding`` :147-190) so the umT5-XXL checkpoint (`models_t5_umt5-xxl-enc-bf16.pth`, key hash
 9c8818c2…) loads unchanged.  The nn.Modules are parameter containers; ``WanTextEncoderEngine`` runs the arithmetic on
-the kernel library: every projection / MLP matrix product on ``svi_gemm_bf16`` (tcgen05), RMS norms, the gated-GELU
+the kernel library: every projection / MLP matrix product on ``svi_gemm_bf16`` (wgmma), RMS norms, the gated-GELU
 product and the 512-token attention with its bucketed relative-position bias and key mask on the encoder kernels
 (``csrc/encoder_kernels.cu``).  No torch compute fallback.
 

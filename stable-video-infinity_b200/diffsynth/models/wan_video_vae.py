@@ -1,4 +1,4 @@
-"""Wan 3-D causal VAE — host side of the B200-native encode/decode at the clip boundaries.
+"""Wan 3-D causal VAE — host side of the H100-native encode/decode at the clip boundaries.
 
 Module / parameter names follow the reference (``diffsynth/models/wan_video_vae.py``: ``WanVideoVAE`` :599-789,
 ``VideoVAE_`` :492-596, ``Encoder3d`` :276-376, ``Decoder3d`` :379-481, ``ResidualBlock`` :198-232,
@@ -8,7 +8,7 @@ checkpoints load unchanged; the nn.Modules only hold parameters.  ``WanVAEEngine
 * activations are channels-last; conv inputs are bf16 *frame rings* ``[slots][H][W][C]`` that keep the last two
   input frames of every causal conv in place (the reference clones / concatenates / pads its feature cache on
   every call, :44-52, :214-232);
-* every conv (3x3x3 causal, 3x3 spatial, (3,1,1) temporal, 1x1x1) is one launch of the tcgen05 implicit-GEMM
+* every conv (3x3x3 causal, 3x3 spatial, (3,1,1) temporal, 1x1x1) is one launch of the wgmma implicit-GEMM
   kernel ``svi_conv3d_causal`` with bias / residual / channel->frame split fused in its epilogue;
 * RMS-norm + SiLU run fused with the fp32 -> bf16 staging of the next conv's input (``svi_vae_norm_act``);
   nearest upsampling and the stride-2 space-to-depth are fused with that staging too;
@@ -20,9 +20,6 @@ The streaming semantics (which conv has which history on which chunk) are those 
 ``oracle/wan_vae_oracle.py``.  Precision: bf16 conv operands, fp32 accumulation, fp32 activations and norms
 (the reference runs the VAE in fp32, svi_video.py:378,386; parity is reported in uint8 levels, DESIGN.md).
 """
-
-import os
-
 import torch
 import torch.nn as nn
 
@@ -141,9 +138,6 @@ class VideoVAE_(nn.Module):
 # ---------------------------------------------------------------------------------------------------------
 def _ceil(a, b):
     return (a + b - 1) // b * b
-
-
-_CONV_VARIANT = int(os.environ.get("SVI_CONV_VARIANT", "0"))
 
 
 def _pick_tile_w(H, W):
@@ -271,8 +265,8 @@ class WanVAEEngine:
 
     # ------------------------------------------------------------------ low-level helpers
     def reset(self):
-        # rings are kept across videos of the same geometry (re-allocating and zero-filling them was 2.5 % of a round trip,
-        # profiles/r02_c7_vae_launches.summary.txt); _ring() replaces one whose geometry changed
+        # rings are kept across videos of the same geometry (re-allocating and zero-filling them every video costs a pass
+        # over every ring); _ring() replaces one whose geometry changed
         for r in self.rings.values():
             r.rewind()
         self.chunk = 0
@@ -323,7 +317,6 @@ class WanVAEEngine:
                 d.slot[t * 3 + a] = slot_table[t][a]
         d.C_out = cv.c_out
         d.tile_w = _pick_tile_w(H, W)
-        d.variant = _CONV_VARIANT          # 0: the library picks (CTA-pair kernel on long rows); 1 / 2 force one kernel (A/B runs)
         if out is not None:
             d.out, d.out_frame_stride, d.out_ld = out.data_ptr(), out_frame_stride, out_ld
         else:
@@ -718,7 +711,7 @@ class WanVideoVAE(nn.Module):
     def _note_untiled(cls, what):
         """`tiled=True` (the pipelines' default argument) is a DOCUMENTED deviation (INTEGRATION.md): the reference's tiling
         (wan_video_vae.py:643-744) is a memory workaround whose blend ramps change the result against its own untiled path;
-        with 180 GB of HBM the untiled computation fits and is what runs.  Said once per process."""
+        with 80 GB of HBM the untiled computation fits and is what runs.  Said once per process."""
         if not cls._tiled_warned:
             cls._tiled_warned = True
             import warnings

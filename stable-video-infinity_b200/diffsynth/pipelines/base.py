@@ -1,6 +1,6 @@
 """Pipeline base: size checks, PIL<->tensor conversion, CPU-generator noise (reference pipelines/base.py).
 
-Residency policy on B200 (180 GB HBM3e): every model stays resident on the device; the reference's
+Residency policy on H100 (80 GB HBM3): every model stays resident on the device; the reference's
 offload / onload choreography (base.py:111-137, vram_management/layers.py) has nothing to do here, so
 ``load_models_to_device`` only makes sure the named models live on ``self.device``.
 """

@@ -1,4 +1,4 @@
-"""SVIVideoPipeline — one clip of the SVI rolling loop on the B200-native kernels.
+"""SVIVideoPipeline — one clip of the SVI rolling loop on the H100-native kernels.
 
 Public surface follows the reference (``diffsynth/pipelines/svi_video.py``: ``SVIVideoPipeline`` :140-520,
 ``model_fn_wan_video`` :74-137) so ``test_svi.py`` can drive it unchanged.  Differences are internal:
@@ -133,8 +133,8 @@ class SVIVideoPipeline(BasePipeline):
 
     # ------------------------------------------------------------------ construction
     def enable_vram_management(self, num_persistent_param_in_dit=None):
-        """Reference svi_video.py:156-241 wraps every Linear for CPU offload under a 6e9-parameter budget.  On a
-        180 GB B200 the whole 14B model (32 GB bf16) plus umT5-XXL, CLIP and the VAE are resident: the all-resident
+        """Reference svi_video.py:156-241 wraps every Linear for CPU offload under a 6e9-parameter budget.  On an
+        80 GB H100 the whole 14B model (32 GB bf16) plus umT5-XXL, CLIP and the VAE are resident: the all-resident
         policy.  The reference harness builds its ModelManager on the CPU (test_svi.py:316-318), so every model the
         pipeline holds is moved here (and in fetch_models): the engines exist for CUDA devices only."""
         for name in ("dit", "vae", "text_encoder", "image_encoder"):

@@ -2,7 +2,7 @@
 
 The reference wraps Linear / conv / norm modules so that weights beyond a parameter budget live on the CPU and
 are re-copied host->device on EVERY forward (layers.py:65-71; ~20 GB per forward for the 14B model under the
-default 6e9 budget, SURVEY.md §8a16).  On a 180 GB B200 everything is resident, so the policy implemented here
+default 6e9 budget, SURVEY.md §8a16).  On an 80 GB H100 everything is resident, so the policy implemented here
 is "all resident": the call is accepted, models are moved to the computation device once, and the module tree
 (whose parameter names are the checkpoint / LoRA key contract) is left untouched.
 """

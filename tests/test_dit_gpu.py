@@ -52,8 +52,8 @@ def test_tiny_dit_matches_oracle(cfg, f, h, w, ctx_len, seed):
             y=None if "y" not in inp else inp["y"].cuda()).float().cpu()
     inside, mx, rel = _stats(out, ref)
     print(f"tiny dit: inside={inside:.4f} max={mx:.4e} mean/std={rel:.4e}")
-    # two blocks of bf16-operand GEMMs: mean |err| ~ 0.07-0.13 % of the output std, 0.948-0.989 inside over the three cases
-    # and runs (round 1, plain bf16 embeddings / patch / head operands: 0.86-0.90 inside, 0.22 %)
+    # two blocks of bf16-operand GEMMs: on an H100, mean |err| 0.07-0.13 % of the output std and 0.953-0.989 inside over the
+    # three cases
     assert inside > 0.93 and mx < 0.012 and rel < 1.6e-3
 
 
@@ -71,7 +71,7 @@ def test_golden_fixture_tiny_t2v():
     inside, mx, rel = _stats(out, torch.from_numpy(g["out"]))
     print(f"golden tiny t2v: inside={inside:.4f} max={mx:.4e} mean/std={rel:.4e}")
     # the fixture was generated from fp32 weights, the engine rounds them to bf16 (what a Wan checkpoint holds): the weight
-    # rounding, not the arithmetic, sets this bar (measured 0.853 / 1.6e-2 / 2.7e-3; with identical weights: test above)
+    # rounding, not the arithmetic, sets this bar (on an H100: 0.854 / 1.6e-2 / 2.7e-3; with identical weights: test above)
     assert inside > 0.82 and mx < 0.025 and rel < 3.5e-3
 
 
@@ -95,7 +95,7 @@ def test_model_fn_and_cfg_euler_step_match_oracle():
     inside, mx, rel = _stats(lat.cpu(), ref)
     print(f"2-step denoise: inside={inside:.4f} max={mx:.4e} mean/std={rel:.4e}")
     # CFG (scale 5) amplifies the per-forward bf16 noise by ~sqrt(5^2 + 4^2) = 6.4x before the Euler update
-    # (measured 0.818 / 3.8e-2 / 2.9e-3; round 1: 0.649 / 5.9e-2 / 5.5e-3)
+    # (on an H100: 0.816 / 2.7e-2 / 2.9e-3)
     assert inside > 0.75 and mx < 0.06 and rel < 4e-3
 
 
@@ -170,7 +170,7 @@ def test_teacache_denoise_matches_oracle():
     assert n_pos.skipped == o_pos.skipped == [1, 2, 4, 6] and n_neg.skipped == o_neg.skipped
     inside, mx, rel = _stats(lat.cpu(), ref)
     print(f"8-step TeaCache denoise: inside={inside:.4f} max={mx:.4e} mean/std={rel:.4e} skipped={n_pos.skipped}")
-    assert inside > 0.80 and rel < 3.5e-3          # measured 0.862 / 2.2e-3
+    assert inside > 0.80 and rel < 3.5e-3          # on an H100: 0.864 / 2.2e-3
 
 
 @pytest.mark.slow
@@ -180,7 +180,7 @@ def test_cfg1_1p3b_one_step_matches_oracle(init, min_inside, max_err, max_rel):
     init="torch_default" is the reference constructors' own initialisation (the survey's 97.5 % / 0.005 bar);
     "normal" is tools.synth's wider N(0, 1/fan_in).  The CPU emulation of bf16 block-GEMM operands alone
     (tools/rounding_study.py `blk`) gives 0.963 / 0.0085 / 1.0e-3 and better than 0.987 / 0.0049 / 7.2e-4.
-    Measured on B200: 0.961 / 0.0107 / 1.03e-3 ("normal") and 1.0000 / 0.0014 / 1.9e-4 ("torch_default")."""
+    """
     from oracle import wan_dit_oracle as O
     cfg = synth.CFG_T2V_1_3B
     sd = {k: v.to(torch.bfloat16).float() for k, v in synth.make_dit_state_dict(cfg, seed=0, init=init).items()}
@@ -224,7 +224,7 @@ def test_block_at_bench_shape_matches_oracle():
     torch.cuda.synchronize()
     inside, mx, rel = _stats(xg.cpu(), ref)
     print(f"block @ L={L}: inside={inside:.5f} max={mx:.4e} mean/std={rel:.4e}")
-    assert inside > 0.999 and mx < 0.008 and rel < 4.5e-4          # measured 0.99990 / 3.2e-3 / 2.9e-4
+    assert inside > 0.999 and mx < 0.008 and rel < 4.5e-4          # on an H100: 0.99991 / 2.9e-3 / 2.9e-4
 
 
 @pytest.mark.slow

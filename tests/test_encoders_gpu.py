@@ -7,7 +7,7 @@ Two yardsticks per encoder, both on bf16-rounded weights:
   * the same oracle with `bf16_points=True`, which rounds exactly where the native path stores bf16 tensors — the
     implementation check: what is left is accumulation order and exp/tanh approximations, so at the tiny sizes >= 85 %
     of the elements must agree to rtol 1e-2 / atol 1e-3 with a mean error below 0.4 % of the standard deviation
-    (measured: 99.7 % / 0.01 %); at the real widths the long fp32 sums flip bf16 roundings and the bound is statistical."""
+    (on an H100: 100 % inside, mean error <= 0.12 % of the std); at the real widths the long fp32 sums flip bf16 roundings and the bound is statistical."""
 import math
 
 import pytest
@@ -138,7 +138,7 @@ def test_umt5_width_two_layers_matches_oracle():
     cfg = dict(SE.TEXT_UMT5_XXL, vocab=1000, num_layers=2)
     out, ref, emu, *_ = _text_case(cfg, 512, 300, 3)
     # K = 4096 / 10240 sums: a different fp32 accumulation order flips bf16 roundings in ~1/3 of the stored elements, so
-    # the bf16-point oracle is only reproduced statistically at this width (measured 0.66 / 5.5e-3)
+    # the bf16-point oracle is only reproduced statistically at this width (on an H100: 0.66 / 5.5e-3)
     _check("umT5-width 2 layers", out, ref, emu, emu_inside=0.5, emu_rel=8e-3)
 
 
@@ -157,4 +157,4 @@ def test_clip_vit_h_width_matches_oracle():
     ref = E.image_encode(sd, cfg, img, SE.CLIP_MEAN, SE.CLIP_STD)
     emu = E.image_encode(sd, cfg, img, SE.CLIP_MEAN, SE.CLIP_STD, bf16_points=True)
     assert out.shape == (1, 257, 1280)
-    _check("CLIP ViT-H width", out, ref, emu, emu_inside=0.7, emu_rel=6e-3)      # measured 0.82 / 2.9e-3
+    _check("CLIP ViT-H width", out, ref, emu, emu_inside=0.7, emu_rel=6e-3)      # on an H100: 0.82 / 2.9e-3

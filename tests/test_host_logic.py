@@ -41,14 +41,15 @@ def test_header_is_plain_c():
     assert r.returncode == 0 and r.stderr.strip() == "", r.stderr
 
 
-def test_library_contains_blackwell_tensor_and_tma_instructions():
-    """SASS evidence that the hot kernels are tcgen05 / TMA code (B200_PROFILING.md: UTC*MMA, LDTM/STTM, UTMALDG)."""
+def test_library_contains_hopper_tensor_and_tma_instructions():
+    """SASS evidence that the hot kernels are wgmma / TMA code for sm_90a (HGMMA, UTMALDG), with no warp-level mma.sync path."""
     from diffsynth import _native as nv
     try:
         sass = subprocess.run(["cuobjdump", "-sass", nv.lib_path()], capture_output=True, text=True, timeout=300).stdout
     except FileNotFoundError:
         pytest.skip("cuobjdump not available")
-    for mnemonic in ("UTCHMMA", "LDTM", "STTM", "UTMALDG"):
+    assert "sm_90a" in subprocess.run(["cuobjdump", "-lelf", nv.lib_path()], capture_output=True, text=True).stdout
+    for mnemonic in ("HGMMA.64x256x16.F32.BF16", "HGMMA.64x128x16.F32.BF16", "UTMALDG"):
         assert mnemonic in sass, f"{mnemonic} not found in the library's SASS"
     assert "HMMA.16816" not in sass       # no legacy mma.sync tensor path
 
@@ -57,22 +58,23 @@ def test_attention_launch_plan_slices_only_the_partial_wave():
     """svi_attn_plan (host logic of svi_attn_fwd): whole units for the full waves, K/V slices for the last partial one."""
     from diffsynth import _native as nv
     big = 1 << 40
-    slice_bytes = 256 * 128 * 4 + 256 * 8
-    # bench shape on one B200: 12 heads x 128 Q-tile pairs = 1536 units = 10.38 waves of 148
-    n_full, split = nv.attention_plan(1536, 256, 148, big)
-    tail = 1536 - n_full
-    assert split > 1 and n_full % 148 == 0 and 0 < tail <= 2 * 148
-    waves = n_full / 148 + -(-tail * split // 148) / split
-    assert waves < 10.75                                            # 11 waves unsliced
-    # sequence-parallel shapes (sp = 2, 4): 5.19 and 2.59 waves
-    for units in (768, 384):
-        nf, sp = nv.attention_plan(units, 256, 148, big)
-        assert sp > 1 and nf / 148 + -(-(units - nf) * sp // 148) / sp < -(-units // 148) - 0.3
-    assert nv.attention_plan(1536, 256, 148, 0) == (1536, 1)        # no workspace: nothing sliced
-    assert nv.attention_plan(1480, 256, 148, big) == (1480, 1)      # exact multiple of the SM count
-    assert nv.attention_plan(1536, 4, 148, big) == (1536, 1)        # cross-attention: K/V stream too short to slice
-    nf, sp = nv.attention_plan(1536, 256, 148, 60 * slice_bytes)    # workspace for 60 slices only
-    assert (1536 - nf) * sp <= 60
+    slice_bytes = 128 * 128 * 4 + 128 * 8
+    # bench shape on one H100 (132 SMs): 12 heads x 256 Q tiles = 3072 units = 23.27 waves
+    n_full, split = nv.attention_plan(3072, 256, 132, big)
+    tail = 3072 - n_full
+    assert split > 1 and n_full % 132 == 0 and 0 < tail <= 2 * 132
+    waves = n_full / 132 + -(-tail * split // 132) / split
+    assert waves < 23.75                                            # 24 waves unsliced
+    # sequence-parallel shape sp = 2: 11.64 waves
+    nf, sp = nv.attention_plan(1536, 256, 132, big)
+    assert sp > 1 and nf / 132 + -(-(1536 - nf) * sp // 132) / sp < -(-1536 // 132) - 0.3
+    # sp = 4: 768 units = 5.82 waves, the last one 82 % full: slicing cannot save 1.5 %, so nothing is sliced
+    assert nv.attention_plan(768, 256, 132, big) == (768, 1)
+    assert nv.attention_plan(3072, 256, 132, 0) == (3072, 1)        # no workspace: nothing sliced
+    assert nv.attention_plan(3036, 256, 132, big) == (3036, 1)      # exact multiple of the SM count
+    assert nv.attention_plan(3072, 4, 132, big) == (3072, 1)        # cross-attention: K/V stream too short to slice
+    nf, sp = nv.attention_plan(3072, 256, 132, 100 * slice_bytes)   # workspace for 100 slices only
+    assert sp > 1 and (3072 - nf) * sp <= 100
 
 
 def test_native_calls_refuse_cpu_tensors():
@@ -444,8 +446,8 @@ def test_ctypes_mirrors_match_the_c_struct_layouts(tmp_path):
 
 
 def test_conv_kernel_choice_is_validated_before_anything_touches_the_gpu():
-    """svi_conv_desc.variant (include/svi_b200.h): 2 = the CTA-pair kernel, which needs k_w = 3 and pad_w = 1; anything outside 0..2 is
-    refused.  The checks run before any tensor map / launch, so the error path is testable without a GPU."""
+    """svi_conv_desc.variant (include/svi_b200.h): kept for ABI compatibility — 2 is accepted only with k_w = 3 and pad_w = 1,
+    anything outside 0..2 is refused (every accepted value runs the same kernel).  The checks run before any tensor map / launch, so the error path is testable without a GPU."""
     from diffsynth import _native as nv
     lib = nv.load()
 

@@ -11,7 +11,7 @@ def test_attention_plan_invariants(units, kv_tiles, sms, ws_slices):
     """svi_attn_plan: whole units + sliced units = all units; slices fit the workspace; slicing never costs more rounds than
     running everything whole; units that fill whole waves are never sliced."""
     from diffsynth import _native as nv
-    slice_bytes = 256 * 128 * 4 + 256 * 8
+    slice_bytes = 128 * 128 * 4 + 128 * 8   # one 128-row Q tile: partial O + (row max, row sum)
     n_full, split = nv.attention_plan(units, kv_tiles, sms, ws_slices * slice_bytes)
     tail = units - n_full
     assert 0 <= n_full <= units and 1 <= split <= 8

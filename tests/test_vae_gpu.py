@@ -1,4 +1,4 @@
-"""GPU parity of the native VAE (tcgen05 implicit-GEMM convs through the C ABI) against the streaming oracle.
+"""GPU parity of the native VAE (wgmma implicit-GEMM convs through the C ABI) against the streaming oracle.
 
 The reference runs the VAE in fp32; the native path uses bf16 conv operands with fp32 accumulation and fp32
 activations, so decode parity is asserted in uint8 pixel levels (what the clip loop actually recycles,

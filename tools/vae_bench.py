@@ -67,8 +67,9 @@ def sweep_from_bench(args):
     pp = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pp):
         peaks = json.load(open(pp))
-    tf_peak = peaks.get("bf16_tflops_sustained", 1400.0)
-    bw_peak = peaks.get("hbm_gbs", peaks.get("hbm_gbps", 6650.0))
+    # without a measured file: NVIDIA's data-sheet figures for the H100 SXM (dense bf16, HBM3), not reached by a power-capped card
+    tf_peak = peaks.get("bf16_tflops_sustained", 989.0)
+    bw_peak = peaks.get("hbm_gbs", peaks.get("hbm_gbps", 3350.0))
     vae = WanVideoVAE().eval()
     vae.load_state_dict(synth_vae.make_vae_state_dict(seed=0))
     vae.to("cuda")
