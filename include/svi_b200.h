@@ -348,6 +348,40 @@ int svi_attn_small(const void* Q, int64_t ldq, const void* K, int64_t ldk, const
                    int64_t ldo, int32_t Lq, int32_t Lk, int32_t num_heads, int32_t head_dim, float scale,
                    const float* bias_table, const int32_t* bucket, const int32_t* key_mask, void* stream);
 
+/*
+ * ---- wav2vec2 audio feature extractor (SVI-Talk audio conditioning, once per audio file) ---------------------------------
+ * Replaces the transformers Wav2Vec2Model that the reference runs on the CPU (utils/src/audio_analysis/wav2vec2.py,
+ * utils/audio_process.py:18-41).  Activations are channels-last [time, channels].  The seven feature-encoder convolutions,
+ * the feature projection, the 16 groups of the positional conv and every encoder projection are svi_gemm_bf16 calls; the
+ * attention is svi_attn_small (head_dim 64); the post-LN steps are svi_layernorm_f32.  These are the remaining ops.
+ *
+ * svi_col_stats         per-column mean and (biased) variance of x f32 [T, ldx] over its T rows, columns [0, C): the
+ *                       GroupNorm with groups = channels after the first conv.  Fixed blocks of rows (their size depends on
+ *                       T only) give fp64 partial sums that a second kernel adds in index order: no atomics, so the same
+ *                       input gives bit-identical statistics on every run and every device.  workspace: 8-byte aligned
+ *                       device scratch of svi_col_stats_workspace_bytes(T, C) bytes (the library never allocates).
+ * svi_col_norm_act      y bf16 [T, ldy] = act((x - mean[c]) * rsqrt(var[c] + eps) * gamma[c] + beta[c]); gamma / beta may
+ *                       be NULL; act: SVI_ACT_*.
+ * svi_conv1d_gather     im2col of a channels-last Conv1d: out bf16 [T_out, ldo] with
+ *                         out[t, j*C + c] = src[t*stride - pad_left + j, col0 + c]   (0 outside [0, T_in)),
+ *                       columns [kernel*C, Kpad) zero; src f32 (src_is_f32) or bf16 [T_in, lds].  The column window
+ *                       [col0, col0 + C) reads one group of a grouped conv in place.  T_out <= (T_in + pad_left + pad_right
+ *                       - kernel) / stride + 1 (a smaller T_out drops trailing outputs).  split != 0: columns
+ *                       [Kpad, 2 Kpad) receive bf16(v - bf16(v)), the two-term form of an f32 operand.  Kpad % 8 == 0.
+ * svi_interp_layernorm  y bf16 [T_out, ldy] = LayerNorm over C of the linear interpolation along time of x f32 [T_in, ldx]
+ *                       (F.interpolate(mode='linear', align_corners=True), torch_utils.py:16-19), affine gamma / beta.
+ */
+size_t svi_col_stats_workspace_bytes(int64_t T, int32_t C);
+int svi_col_stats(const float* x, int64_t ldx, int64_t T, int32_t C, float* mean, float* var, void* workspace,
+                  size_t workspace_bytes, void* stream);
+int svi_col_norm_act(const float* x, int64_t ldx, int64_t T, int32_t C, const float* mean, const float* var, float eps,
+                     const float* gamma, const float* beta, int32_t act, void* y_bf16, int64_t ldy, void* stream);
+int svi_conv1d_gather(const void* src, int32_t src_is_f32, int64_t lds, int64_t T_in, int32_t col0, int32_t C,
+                      int32_t kernel, int32_t stride, int32_t pad_left, int32_t pad_right, int64_t T_out, int32_t split,
+                      void* out_bf16, int64_t ldo, int32_t Kpad, void* stream);
+int svi_interp_layernorm(const float* x, int64_t ldx, int64_t T_in, int32_t C, int64_t T_out, float eps,
+                         const float* gamma, const float* beta, void* y_bf16, int64_t ldy, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

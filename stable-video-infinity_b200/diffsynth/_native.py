@@ -97,6 +97,11 @@ SIGNATURES = {
     "svi_vae_to_planar": (_i32, [_vp, _i64, _i32, _i64, _vp, _vp, _i32, _vp, _i64, _vp]),
     "svi_softmax_rows": (_i32, [_vp, _i32, _i32, _i64, _f32, _vp, _i64, _vp]),
     "svi_frames_to_uint8": (_i32, [_vp, _i64, _i64, _vp, _vp]),
+    "svi_col_stats_workspace_bytes": (_c.c_size_t, [_i64, _i32]),
+    "svi_col_stats": (_i32, [_vp, _i64, _i64, _i32, _vp, _vp, _vp, _c.c_size_t, _vp]),
+    "svi_col_norm_act": (_i32, [_vp, _i64, _i64, _i32, _vp, _vp, _f32, _vp, _vp, _i32, _vp, _i64, _vp]),
+    "svi_conv1d_gather": (_i32, [_vp, _i32, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i64, _i32, _vp, _i64, _i32, _vp]),
+    "svi_interp_layernorm": (_i32, [_vp, _i64, _i64, _i32, _i64, _f32, _vp, _vp, _vp, _i64, _vp]),
 }
 
 _lib = None
@@ -603,3 +608,62 @@ def softmax_rows(s, N, scale, p):
                                  _ptr(p, torch.bfloat16, "p"), _rowmajor(p, "p"), _stream())
     _check(rc, "svi_softmax_rows")
     return p
+
+
+# --------------------------------------------------------------------------------------------- wav2vec2 audio encoder
+def col_stats_workspace_bytes(T, C):
+    return int(load().svi_col_stats_workspace_bytes(int(T), int(C)))
+
+
+def col_stats(x, mean, var, workspace):
+    """mean / var f32 [C] = per-column mean and biased variance of x f32 [T, C] (row-strided view allowed) over its rows;
+    reproducible (fixed-order fp64 reduction).  workspace: CUDA tensor of >= col_stats_workspace_bytes(T, C) bytes."""
+    T, C = x.shape
+    if mean.numel() != C or var.numel() != C or not mean.is_contiguous() or not var.is_contiguous():
+        raise RuntimeError("svi_b200.col_stats: mean and var must be contiguous [C]")
+    if not workspace.is_cuda or not workspace.is_contiguous():
+        raise RuntimeError("svi_b200.col_stats: workspace must be a contiguous CUDA tensor")
+    rc = load().svi_col_stats(_ptr(x, torch.float32, "x"), _rowmajor(x, "x"), T, C, _ptr(mean, torch.float32, "mean"),
+                              _ptr(var, torch.float32, "var"), _vp(workspace.data_ptr()),
+                              workspace.numel() * workspace.element_size(), _stream())
+    _check(rc, "svi_col_stats")
+
+
+def col_norm_act(x, mean, var, eps, gamma, beta, act, out):
+    """out bf16 [T, C] = act((x - mean) * rsqrt(var + eps) * gamma + beta), per column (row-strided views allowed)."""
+    T, C = x.shape
+    if tuple(out.shape) != (T, C):
+        raise RuntimeError("svi_b200.col_norm_act: out must be [T, C]")
+    rc = load().svi_col_norm_act(_ptr(x, torch.float32, "x"), _rowmajor(x, "x"), T, C, _ptr(mean, torch.float32, "mean"),
+                                 _ptr(var, torch.float32, "var"), float(eps), _ptr(gamma, torch.float32, "gamma"),
+                                 _ptr(beta, torch.float32, "beta"), int(act), _ptr(out, torch.bfloat16, "out"),
+                                 _rowmajor(out, "out"), _stream())
+    _check(rc, "svi_col_norm_act")
+    return out
+
+
+def conv1d_gather(src, out, kernel, stride, pad_left=0, pad_right=0, col0=0, C=None, split=False):
+    """im2col of a channels-last Conv1d: out bf16 [T_out, >= Kpad (2 Kpad with split)] (tap, channel) columns of the
+    column window [col0, col0 + C) of src f32 / bf16 [T_in, ld]; T_out = out.shape[0], Kpad = out.shape[1] (/ 2 with split)."""
+    T_in, width = src.shape
+    C = width - col0 if C is None else C
+    if src.dtype not in (torch.float32, torch.bfloat16) or src.stride(1) != 1 or col0 + C > width:
+        raise RuntimeError("svi_b200.conv1d_gather: src must be f32 or bf16 with unit inner stride and col0 + C <= width")
+    kpad = out.shape[1] // (2 if split else 1)
+    rc = load().svi_conv1d_gather(_ptr(src, name="src"), int(src.dtype == torch.float32), src.stride(0), T_in, int(col0), int(C),
+                                  int(kernel), int(stride), int(pad_left), int(pad_right), out.shape[0], int(bool(split)),
+                                  _ptr(out, torch.bfloat16, "out"), _rowmajor(out, "out"), kpad, _stream())
+    _check(rc, "svi_conv1d_gather")
+    return out
+
+
+def interp_layernorm(x, T_out, gamma, beta, eps, out):
+    """out bf16 [T_out, C] = LayerNorm(linear_interpolation(x f32 [T_in, C], T_out)) * gamma + beta."""
+    T_in, C = x.shape
+    if out.shape[0] != T_out or out.shape[1] != C:
+        raise RuntimeError("svi_b200.interp_layernorm: out must be [T_out, C]")
+    rc = load().svi_interp_layernorm(_ptr(x, torch.float32, "x"), _rowmajor(x, "x"), T_in, C, int(T_out), float(eps),
+                                     _ptr(gamma, torch.float32, "gamma"), _ptr(beta, torch.float32, "beta"),
+                                     _ptr(out, torch.bfloat16, "out"), _rowmajor(out, "out"), _stream())
+    _check(rc, "svi_interp_layernorm")
+    return out

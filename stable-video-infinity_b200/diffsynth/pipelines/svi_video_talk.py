@@ -8,9 +8,12 @@ into a first-frame window and per-latent-frame windows (`preprocess_audio`, :432
     v = v_uncond + s_text * (v_cond - v_drop_text) + s_audio * (v_drop_text - v_uncond)
 
 with v_cond (prompt, audio), v_drop_text (negative prompt, audio), v_uncond (negative prompt, silent audio).
-The wav2vec2 feature extractor is an external model (`utils/src/audio_analysis` in the reference, not part of diffsynth):
-pass its output as `audio_embed`; `audio_path` alone raises.
+The clip's window features come either from `audio_embed=` or, as in the reference, from `audio_path=`: the wav2vec2
+extractor (diffsynth.models.wav2vec2, loaded from `wav2vec_path` on first use) runs on the GPU once per audio file, and
+every clip of a video gathers its windows from the cached [T, 12, 768] hidden states.
 """
+import os
+
 import torch
 from PIL import Image
 from tqdm import tqdm
@@ -50,12 +53,17 @@ def model_fn_wan_talk_video(dit, x, timestep, context, clip_feature=None, y=None
 
 
 class SVITalkVideoPipeline(SVIVideoPipeline):
-    def __init__(self, device="cuda", torch_dtype=torch.float16, tokenizer_path=None, wav2vec_path=None, is_test=False):
+    def __init__(self, device="cuda", torch_dtype=torch.float16, tokenizer_path=None, wav2vec_path="./weights/chinese-wav2vec2-base/",
+                 is_test=False):
         super().__init__(device=device, torch_dtype=torch_dtype, tokenizer_path=tokenizer_path, is_test=is_test)
         self.wav2vec_path = wav2vec_path
+        self.wav2vec_feature_extractor, self.audio_encoder = None, None
+        self._audio_cache = None           # ((real path, size, mtime), [T, 12, 768] f32 on the device)
+        self.audio_extractions = 0
 
     @staticmethod
-    def from_model_manager(model_manager, torch_dtype=None, device=None, use_usp=False, is_test=False, wav2vec_path=None):
+    def from_model_manager(model_manager, torch_dtype=None, device=None, use_usp=False, is_test=False,
+                           wav2vec_path="./weights/chinese-wav2vec2-base/"):
         device = model_manager.device if device is None else device
         torch_dtype = model_manager.torch_dtype if torch_dtype is None else torch_dtype
         pipe = SVITalkVideoPipeline(device=device, torch_dtype=torch_dtype, wav2vec_path=wav2vec_path, is_test=is_test)
@@ -64,10 +72,42 @@ class SVITalkVideoPipeline(SVIVideoPipeline):
             pipe.enable_usp()
         return pipe
 
+    def load_audio_encoder(self):
+        """reference custom_init (:26-30): the wav2vec2 model and its feature extractor from `wav2vec_path`, on the
+        pipeline's device (the reference keeps them on the CPU)."""
+        if self.audio_encoder is None:
+            from ..models.wav2vec2 import Wav2Vec2FeatureExtractor, Wav2Vec2Model
+            path = self.wav2vec_path
+            if path is None or not os.path.isdir(path):
+                raise FileNotFoundError(f"SVI-Talk: wav2vec2 model directory {path!r} not found (config.json, "
+                                        f"preprocessor_config.json and model.safetensors / pytorch_model.bin); pass "
+                                        f"wav2vec_path= or the window features as audio_embed=")
+            self.wav2vec_feature_extractor = Wav2Vec2FeatureExtractor.from_pretrained(path)
+            self.audio_encoder = Wav2Vec2Model.from_pretrained(path)
+        return self.wav2vec_feature_extractor, self.audio_encoder
+
+    def audio_hidden_states(self, audio_path):
+        """[T, 12, 768] f32 wav2vec2 features of a whole audio file at 25 fps, on the device.  Cached by (real path, size,
+        mtime), so the clips of one video share one extraction.  Every rank of a sequence-parallel run extracts on its own;
+        the reductions are deterministic, so all ranks hold identical features."""
+        from utils.audio_process import audio_prepare_single, get_embedding
+        st = os.stat(audio_path)
+        key = (os.path.realpath(audio_path), st.st_size, st.st_mtime_ns)
+        if self._audio_cache is None or self._audio_cache[0] != key:
+            fe, enc = self.load_audio_encoder()
+            speech = audio_prepare_single(audio_path, fe.sampling_rate)
+            emb = get_embedding(speech, fe, enc, sr=fe.sampling_rate, device=self.device)
+            self.audio_extractions += 1
+            self._audio_cache = (key, emb)
+        return self._audio_cache[1]
+
     def get_audio_embedding(self, audio_path, num_frames, audio_start_idx=0):
-        raise NotImplementedError(
-            "svi_b200: wav2vec2 feature extraction is not part of this package (the reference uses its own "
-            "utils/src/audio_analysis model); pass the [1, num_frames, 5, 12, 768] window features as audio_embed=")
+        """reference :412-430: 5-frame windows centred on audio_start_idx .. audio_start_idx + num_frames - 1, indices
+        clamped to [0, T-1] -> [1, num_frames, 5, 12, 768] f32 on the device."""
+        emb = self.audio_hidden_states(audio_path)
+        idx = torch.arange(audio_start_idx, audio_start_idx + num_frames).unsqueeze(1) + (torch.arange(5) - 2).unsqueeze(0)
+        idx = idx.clamp(0, emb.shape[0] - 1).to(emb.device)
+        return emb[idx][None]
 
     def preprocess_audio(self, audio_embed, audio_window=5, vae_scale=4):
         first, latter = preprocess_audio(audio_embed, audio_window, vae_scale)
