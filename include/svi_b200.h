@@ -334,7 +334,8 @@ int svi_softmax_rows(const float* s, int32_t rows, int32_t N, int64_t lds, float
  *                       Q,K,V,O bf16 [L, ld] with head h at columns [h*head_dim, (h+1)*head_dim);
  *                       bias_table f32 [n_buckets, H] + bucket int32 [Lq, Lk] (T5RelativeEmbedding :159-190, the
  *                       bucket of (query, key) is position-only and shared by all layers) or both NULL;
- *                       key_mask int32 [Lk] (0 = masked; T5Attention :73-77) or NULL.
+ *                       key_mask int32 [Lk] (0 = masked; T5Attention :73-77) or NULL; with every key masked the
+ *                       output rows are 0 (not the NaN of a softmax over an empty set).
  *                       Replaces T5Attention.forward :55-89 (scale 1, bias, mask) and the CLIP SelfAttention
  *                       (wan_video_image_encoder.py:255-268: head_dim 80, scale 1/sqrt(80)).
  */

@@ -13,7 +13,9 @@ import torch.nn.functional as F
 
 def _act(v, act):
     if act == 1:
-        return F.gelu(v, approximate="tanh")
+        # in fp64: torch's fp32 0.5 x (1 + tanh(u)) cancels for x < -2 (a bf16 ulp off in a quarter of those elements, 0 below
+        # about -5.5), while the kernels' x * sigmoid(2u) keeps ~1e-6 relative accuracy
+        return F.gelu(v.double(), approximate="tanh").to(v.dtype)
     if act == 2:
         return F.silu(v)
     if act == 3:

@@ -16,9 +16,12 @@ def layernorm_f32(x, gamma, beta, eps, out):
 
 
 def attention_small(q, k, v, out, num_heads, head_dim, scale, bias_table=None, bucket=None, key_mask=None):
-    assert bias_table is None and bucket is None and key_mask is None
+    assert bias_table is None and bucket is None
     qf, kf, vf = (t.float().reshape(t.shape[0], num_heads, head_dim).transpose(0, 1) for t in (q, k, v))
-    o = torch.softmax(qf @ kf.transpose(-1, -2) * scale, dim=-1) @ vf           # fp32 throughout (SIMT kernel)
+    s = qf @ kf.transpose(-1, -2) * scale
+    if key_mask is not None:
+        s = s.masked_fill(key_mask.view(1, 1, -1) == 0, float("-inf"))
+    o = torch.softmax(s, dim=-1).nan_to_num(0.0) @ vf      # fp32 throughout (SIMT kernel); every key masked -> 0
     out.copy_(o.transpose(0, 1).reshape(q.shape[0], num_heads * head_dim).to(out.dtype))
     return out
 

@@ -6,7 +6,9 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("section", ["gemm", "gemm_epi", "attn", "attn_cross", "attn_bench", "abi3", "ln_fold", "ew", "conv"])
+@pytest.mark.parametrize("section", ["gemm", "gemm_epi", "attn", "attn_cross", "attn_bench", "abi3", "ln_fold", "ew", "conv",
+                                     "conv_tiles", "gemm_edges", "attn_online", "attn_sp_one_gpu",
+                                     pytest.param("attn_sp_one_gpu_long", marks=pytest.mark.slow), "attn_small_long"])
 def test_kernel_section(section):
     from tools import gpu_check as G
     G.RESULTS.clear()

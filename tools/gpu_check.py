@@ -1,7 +1,9 @@
 """Kernel-level GPU checks with verbose diagnostics (development tool; the pytest -m gpu suite is the gate).
 
-usage: python tools/gpu_check.py <section> [...]   sections: gemm gemm_epi attn attn_cross ew perf_gemm perf_attn
-Each section prints one line per case: name, max abs err, reference scale, verdict.
+usage: python tools/gpu_check.py <section> [...]   sections: every sec_<name> below, e.g. gemm gemm_edges attn attn_online
+       attn_sp_one_gpu conv conv_tiles ew perf_gemm perf_attn
+Each section prints one line per case: name, max abs err, reference scale, verdict.  A "negative control" case passes when
+a wrong but plausible reference fails the bar, i.e. when the bar is sharp enough to tell the two apart.
 """
 import math
 import os
@@ -18,19 +20,35 @@ dev = "cuda"
 RESULTS = []   # (name, ok) of every report() call — tests/test_kernels_gpu.py asserts on it
 
 
+def _bar(got, ref, tol, min_inside):
+    """(ok, max err, max |ref|, fraction inside the elementwise tolerance, err) of report()'s bar"""
+    got = got.float()
+    ref = ref.float()
+    err = (got - ref).abs()
+    mx = err.max().item()
+    scale = ref.abs().max().item()
+    rms = ref.pow(2).mean().sqrt().item()
+    inside = (err <= 1e-3 * rms + 1e-2 * ref.abs()).float().mean().item()
+    ok = math.isfinite(mx) and mx <= tol * max(scale, 1e-6) and (min_inside is None or inside >= min_inside)
+    return ok, mx, scale, inside, err
+
+
+def negative(name, got, wrong, tol, min_inside=None):
+    """Negative control of report(): a wrong but plausible reference must FAIL the same bar (recorded as a case)."""
+    ok_wrong, mx, _, inside, _ = _bar(got, wrong, tol, min_inside)
+    print(f"[{'BAD' if ok_wrong else 'OK '}] negative control {name}: the wrong reference "
+          f"{'passes' if ok_wrong else 'fails'} the bar (max_err={mx:.4e} inside={inside:.4f})", flush=True)
+    RESULTS.append((f"negative control {name}", not ok_wrong))
+
+
 def report(name, got, ref, tol, min_inside=None):
     """Max-norm criterion (err <= tol * max|ref|) and, when min_inside is given, the elementwise criterion of the north
     star as well: the fraction of elements with err <= 1e-3 * rms(ref) + 1e-2 * |ref| must reach min_inside (atol is taken
     relative to the reference's rms so that the bar means the same for unit-scale and for 1/sqrt(L)-scale outputs)."""
     got = got.float()
     ref = ref.float()
-    err = (got - ref).abs()
-    mx = err.max().item()
-    scale = ref.abs().max().item()
+    ok, mx, scale, inside, err = _bar(got, ref, tol, min_inside)
     bad = (err > tol * max(scale, 1e-6)).float().mean().item()
-    rms = ref.pow(2).mean().sqrt().item()
-    inside = (err <= 1e-3 * rms + 1e-2 * ref.abs()).float().mean().item()
-    ok = math.isfinite(mx) and mx <= tol * max(scale, 1e-6) and (min_inside is None or inside >= min_inside)
     print(f"[{'OK ' if ok else 'BAD'}] {name}: max_err={mx:.4e} ref_max={scale:.4e} frac_bad={bad:.4f} "
           f"inside(rtol 1e-2, atol 1e-3 rms)={inside:.4f}", flush=True)
     RESULTS.append((name, ok))
@@ -159,6 +177,27 @@ def attn_ref(q, k, v, H, scale):
     s = (qh @ kh.transpose(1, 2)) * scale
     p = torch.softmax(s, dim=-1)
     return (p @ vh).transpose(0, 1).reshape(Lq, H * 128)
+
+
+def attn_ref_no_rescale(q, k, v, H, scale, hd=128, tile=128, first_tile=0):
+    """A WRONG online softmax for negative controls: K/V tiles in the kernel's visiting order (starting at first_tile,
+    wrapping), the running max updated per tile, but the accumulated O and row sum never rescaled by exp(m_old - m_new)."""
+    Lq, Lk = q.shape[0], k.shape[0]
+    qh = q.float().view(Lq, H, hd).transpose(0, 1)
+    kh = k.float().view(Lk, H, hd).transpose(0, 1)
+    vh = v.float().view(Lk, H, hd).transpose(0, 1)
+    n = (Lk + tile - 1) // tile
+    m = torch.full((H, Lq, 1), float("-inf"), device=q.device)
+    l = torch.zeros(H, Lq, 1, device=q.device)
+    o = torch.zeros(H, Lq, hd, device=q.device)
+    for j in range(n):
+        t = (j + first_tile) % n
+        s = (qh @ kh[:, t * tile:(t + 1) * tile].transpose(1, 2)) * scale
+        m = torch.maximum(m, s.amax(-1, keepdim=True))
+        p = torch.exp(s - m)
+        l = l + p.sum(-1, keepdim=True)
+        o = o + p @ vh[:, t * tile:(t + 1) * tile]
+    return (o / l).transpose(0, 1).reshape(Lq, H * hd)
 
 
 def sec_attn():
@@ -446,6 +485,221 @@ def sec_ew():
     report("add_rows bcast", oo[:2], tb[:2] + tt[:1], 1e-6)
 
 
+def _gemm_bound_report(name, got, a, w, K, bias=None, act=0, gate=None, residual=None, c=2.0, drop_tail=True):
+    """Per-element bar of a GEMM against its fp64 reference: |err| <= c K 2^-24 (|A| |W|^T)[m, n] (accumulation), plus a few
+    fp32 roundings of the epilogue terms, plus half a bf16 ulp of the value for bf16 outputs.  Negative control: the reference
+    without the last 8 columns of K (a K tail read as zero) must fail it."""
+    def ref_of(kk):
+        v = a[:, :kk].double() @ w[:, :kk].double().t()
+        if bias is not None:
+            v = v + bias.double()
+        if act == nv.ACT_RELU:
+            v = v.clamp_min(0)
+        if gate is not None:
+            v = v * gate.double()
+        if residual is not None:
+            v = v + residual.double()
+        return v
+    ref = ref_of(K)
+    P = a.double().abs() @ w.double().abs().t()
+    g_abs = gate.double().abs() if gate is not None else 1.0
+    epi = (bias.double().abs() if bias is not None else 0.0) * g_abs + (residual.double().abs() if residual is not None else 0.0)
+    bound = 2.0 ** -24 * (c * K * P * g_abs + 4 * (epi + ref.abs()))
+    gotd = got.double()
+    if got.dtype == torch.bfloat16:
+        _, e = torch.frexp(torch.maximum(gotd.abs(), ref.abs()))
+        bound = bound + torch.ldexp(torch.full_like(bound, 0.5), e - 8)      # half a bf16 ulp
+    err = (gotd - ref).abs()
+    inside = err <= bound
+    ok = bool(inside.all())
+    worst = (err / bound.clamp_min(1e-300)).max().item()
+    print(f"[{'OK ' if ok else 'BAD'}] {name}: max_err={err.max().item():.3e} worst err/bound={worst:.3f} (c={c})", flush=True)
+    RESULTS.append((name, ok))
+    if not ok:
+        r, cc = (~inside).nonzero()[0].tolist()
+        print(f"      first outside [{r},{cc}] got={gotd[r, cc].item()} ref={ref[r, cc].item()} bound={bound[r, cc].item():.3e}")
+    if drop_tail and K > 8:
+        caught = not bool(((gotd - ref_of(K - 8)).abs() <= bound).all())
+        print(f"[{'OK ' if caught else 'BAD'}] negative control {name}: reference without the last 8 K columns fails: {caught}", flush=True)
+        RESULTS.append((f"negative control {name}", caught))
+    return ref
+
+
+def sec_gemm_edges():
+    """GEMM edges under a per-element fp64 bound: ReLU epilogue, A and W as column slices of NaN-padded wider buffers
+    (lda / ldw > K, K % 64 != 0: the tensor-map extent must zero-fill, not read the neighbours), bf16 out with gate + f32
+    residual, N = 8 / 264, M = 1, 32-column atomic sumsq groups, and more than 2 x 132 tiles so every CTA loops.
+    Measured on an H100 80GB HBM3 at a 400 W power limit: f32 outputs use at most 9 % of the c = 2 bound (K = 8; under 2 %
+    for K >= 72); bf16 outputs up to 99.8 %, which is the half-ulp rounding term."""
+    g = torch.Generator(device="cpu").manual_seed(31)
+
+    def operands(M, N, K, pad=0):
+        a_big = torch.full((M, K + pad), float("nan"), dtype=torch.bfloat16, device=dev)
+        w_big = torch.full((N, K + pad), float("nan"), dtype=torch.bfloat16, device=dev)
+        a_big[:, :K] = (torch.randn(M, K, generator=g) * 0.5).to(dev, torch.bfloat16)
+        w_big[:, :K] = (torch.randn(N, K, generator=g) * 0.5).to(dev, torch.bfloat16)
+        return a_big[:, :K], w_big[:, :K]
+
+    for (M, N, K, pad) in [(300, 264, 8, 56), (130, 264, 72, 8), (257, 520, 200, 24), (1, 8, 72, 40), (1, 264, 200, 0),
+                           (129, 8, 8, 8)]:
+        a, w = operands(M, N, K, pad)
+        out = torch.full((M, N), float("nan"), device=dev)
+        nv.gemm(a, w, out)
+        _gemm_bound_report(f"gemm_edges f32 M={M} N={N} K={K} lda=ldw={K + pad}", out, a, w, K)
+    # ReLU epilogue (AudioProjModel), f32 and bf16 out
+    M, N, K = 300, 264, 200
+    a, w = operands(M, N, K, 24)
+    bias = torch.randn(N, generator=g).to(dev)
+    for dt in (torch.float32, torch.bfloat16):
+        out = torch.full((M, N), float("nan"), device=dev, dtype=dt)
+        nv.gemm(a, w, out, bias=bias, act=nv.ACT_RELU)
+        _gemm_bound_report(f"gemm_edges bias+relu {dt}", out, a, w, K, bias=bias, act=nv.ACT_RELU)
+        negative(f"gemm_edges relu {dt}: reference without the ReLU", out, a.float() @ w.float().t() + bias, 2e-3)
+    # bf16 out with gate + f32 residual, into a column slice of a wider buffer
+    gate = torch.randn(N, generator=g).to(dev)
+    res = torch.randn(M, N, generator=g).to(dev)
+    big = torch.full((M, N + 40), float("nan"), device=dev, dtype=torch.bfloat16)
+    nv.gemm(a, w, big[:, :N], bias=bias, gate=gate, residual=res)
+    _gemm_bound_report("gemm_edges bf16 out bias+gate+residual", big[:, :N], a, w, K, bias=bias, gate=gate, residual=res)
+    RESULTS.append(("gemm_edges bf16 out: columns beyond N untouched", bool(torch.isnan(big[:, N:].float()).all())))
+    # 32-column atomic sumsq groups (7 of the 8 groups accumulated)
+    N2 = 256
+    a2, w2 = operands(M, N2, K, 8)
+    b2 = torch.randn(N2, generator=g).to(dev)
+    ss = torch.zeros(M, 7, device=dev)
+    out = torch.full((M, N2), float("nan"), device=dev)
+    nv.gemm(a2, w2, out, bias=b2, sumsq=ss, sumsq_group_cols=32)
+    v = _gemm_bound_report("gemm_edges f32 with 32-column sumsq groups", out, a2, w2, K, bias=b2)
+    want = (v[:, :224] ** 2).reshape(M, 7, 32).sum(2)
+    P = (a2.double().abs() @ w2.double().abs().t() + b2.double().abs())[:, :224]
+    ss_bound = (2 * v[:, :224].abs() * 2.0 ** -24 * (2 * K * P + 4 * v[:, :224].abs())).reshape(M, 7, 32).sum(2) \
+        + 2.0 ** -24 * 64 * want
+    err = (ss.double() - want).abs()
+    ok = bool((err <= ss_bound).all())
+    print(f"[{'OK ' if ok else 'BAD'}] gemm_edges sumsq 32-column groups: worst err/bound={(err / ss_bound).max().item():.3f}", flush=True)
+    RESULTS.append(("gemm_edges sumsq 32-column groups", ok))
+    wrong_ss = (v[:, :256] ** 2).reshape(M, 8, 32).sum(2)[:, 1:]          # groups shifted by one
+    RESULTS.append(("negative control gemm_edges sumsq: shifted groups fail", not bool(((ss.double() - wrong_ss).abs() <= ss_bound).all())))
+    # more than 2 x 132 output tiles: every persistent CTA takes several
+    a3, w3 = operands(2048, 4608, 136, 8)
+    out = torch.full((2048, 4608), float("nan"), device=dev, dtype=torch.bfloat16)
+    nv.gemm(a3, w3, out)
+    _gemm_bound_report("gemm_edges bf16 M=2048 N=4608 K=136 (every CTA loops)", out, a3, w3, 136)
+
+
+def sec_attn_online():
+    """Online softmax under stress (bar: report()'s elementwise min_inside against the fp32 reference): key amplitude
+    growing along the sequence so the row max rises in every K/V tile, one dominant key in the last tile or in a middle slice
+    of a sliced plan, Lk = 1 / 129, Lq = 1, score std 10-20, with and without workspace.  Negative control: the same online
+    softmax without the exp(m_old - m_new) rescale."""
+    g = torch.Generator(device="cpu").manual_seed(32)
+    scale = 128 ** -0.5
+
+    def make(Lq, Lk, H, amp, ramp=0.0, dominant=None):
+        q = torch.randn(Lq, H * 128, generator=g) * amp
+        k = torch.randn(Lk, H * 128, generator=g) * amp
+        v = torch.randn(Lk, H * 128, generator=g)
+        q.view(Lq, H, 128)[:, :, 0] = 4.0                   # a common direction: scores rise with k[:, 0]
+        k.view(Lk, H, 128)[:, :, 0] += ramp * torch.arange(Lk).float().unsqueeze(1) / max(Lk - 1, 1)
+        if dominant is not None:
+            k.view(Lk, H, 128)[dominant, :, 0] = 100.0     # +35 on every score of that key
+        return (t.to(dev, torch.bfloat16) for t in (q, k, v))
+
+    cases = [("ramp", 1000, 1000, 2, 3.5, 120.0, None), ("ramp sliced", 3200, 4100, 12, 3.5, 120.0, None),
+             ("dominant key in the last tile", 700, 1000, 2, 3.2, 0.0, 999),
+             ("dominant key in a middle slice", 3200, 4100, 12, 3.2, 0.0, 2053),
+             ("Lk=1", 300, 1, 2, 3.5, 0.0, None), ("Lk=129", 300, 129, 3, 3.5, 50.0, 128), ("Lq=1", 1, 1000, 2, 3.5, 120.0, None),
+             ("std 20", 513, 777, 2, 4.5, 0.0, None)]
+    for name, Lq, Lk, H, amp, ramp, dom in cases:
+        q, k, v = make(Lq, Lk, H, amp, ramp, dom)
+        ref = attn_ref(q, k, v, H, scale)
+        wrong = attn_ref_no_rescale(q, k, v, H, scale)
+        s_std = (q.float()[:, :128] @ k.float()[:, :128].t() * scale).std().item()
+        for ws in (None, torch.empty(nv.attention_workspace_bytes(Lq, Lk, H) // 4 + 1, device=dev)):
+            out = torch.full((Lq, H * 128), float("nan"), device=dev, dtype=torch.bfloat16)
+            nv.attention(q, k, v, out, H, scale, workspace=ws)
+            torch.cuda.synchronize()
+            tag = f"attn_online {name} Lq={Lq} Lk={Lk} H={H} score std {s_std:.1f} workspace={'yes' if ws is not None else 'no'}"
+            report(tag, out, ref, 2e-2, min_inside=0.99)
+            if Lk > 128:
+                negative(tag + " (no rescale)", out, wrong, 2e-2, min_inside=0.99)
+
+
+def _attn_sp_cases(shapes):
+    """svi_attn_fwd_sp on one GPU: every flag already holds the epoch (set and synchronised before the launch), so the
+    producer never waits; what runs is the K/V stream that starts on the local chunk and wraps, the ragged last tile visited
+    mid-stream, sliced units offset by kv_first_tile and the merge of the slices."""
+    g = torch.Generator(device="cpu").manual_seed(33)
+    scale = 128 ** -0.5
+    epoch = 5
+    for (L, chunk, H, amp) in shapes:
+        q = (torch.randn(L, H * 128, generator=g) * amp).to(dev, torch.bfloat16)
+        k = (torch.randn(L, H * 128, generator=g) * amp).to(dev, torch.bfloat16)
+        v = torch.randn(L, H * 128, generator=g).to(dev, torch.bfloat16)
+        ref = attn_ref_chunked(q, k, v, H, scale) if L > 8192 else attn_ref(q, k, v, H, scale)
+        n_chunks = (L + chunk - 1) // chunk
+        flags = torch.full((n_chunks,), epoch, dtype=torch.int32, device=dev)
+        torch.cuda.synchronize()                          # the flags hold the epoch before any launch reads them
+        for c in range(n_chunks):
+            r0, r1 = c * chunk, min(L, (c + 1) * chunk)
+            ql = q[r0:r1]
+            plain = torch.empty(r1 - r0, H * 128, device=dev, dtype=torch.bfloat16)
+            nv.attention(ql, k, v, plain, H, scale)
+            first_tile = (c * chunk + 127) // 128
+            for ws in (None, torch.empty(nv.attention_workspace_bytes(r1 - r0, L, H) // 4 + 1, device=dev)):
+                out = torch.full((r1 - r0, H * 128), float("nan"), device=dev, dtype=torch.bfloat16)
+                nv.attention_sp(ql, k, v, out, H, flags, epoch, chunk, c, scale, workspace=ws)
+                torch.cuda.synchronize()
+                tag = f"attn_sp one GPU L={L} chunk={chunk} H={H} self_chunk={c} workspace={'yes' if ws is not None else 'no'}"
+                report(tag, out, ref[r0:r1], 2e-2, min_inside=0.95)
+                report(tag + " vs attention()", out, plain, 2e-2)
+            if c == n_chunks - 1:
+                negative(f"attn_sp L={L} self_chunk={c} (no rescale)", out,
+                         attn_ref_no_rescale(ql, k, v, H, scale, first_tile=first_tile), 2e-2, min_inside=0.95)
+
+
+def sec_attn_sp_one_gpu():
+    # L = 1260 in two 630-row chunks (chunk boundaries inside a K/V tile, ragged 108-row last tile); L = 4100 in two chunks:
+    # 34 units on 132 SMs, so the workspace plan slices every unit and the slices start at j_begin + kv_first_tile
+    _attn_sp_cases([(1260, 630, 2, 2.0), (4100, 2050, 2, 2.0), (1260, 420, 3, 2.0)])
+
+
+def sec_attn_sp_one_gpu_long():
+    # the benchmark shape on 4 ranks: L = 32760 in 8190-row chunks, 12 heads
+    _attn_sp_cases([(32760, 8190, 12, 2.0)])
+
+
+def sec_attn_small_long():
+    """svi_attn_small at the wav2vec2 length (61 s at 50 Hz: ~3050 tokens, 12 heads x 64) against fp32, and a key mask.
+    A launch whose keys are all masked writes 0 (header: svi_attn_small)."""
+    g = torch.Generator(device="cpu").manual_seed(34)
+    L, H, hd = 3050, 12, 64
+    scale = hd ** -0.5
+    q, k, v = ((torch.randn(L, H * hd, generator=g) * a).to(dev, torch.bfloat16) for a in (2.0, 2.0, 1.0))
+
+    def ref_of(mask=None):
+        qh, kh, vh = (t.float().view(L, H, hd).transpose(0, 1) for t in (q, k, v))
+        s = qh @ kh.transpose(1, 2) * scale
+        if mask is not None:
+            s = s.masked_fill(mask.view(1, 1, L) == 0, float("-inf"))
+        return (torch.softmax(s, -1) @ vh).transpose(0, 1).reshape(L, H * hd)
+
+    out = torch.full((L, H * hd), float("nan"), device=dev, dtype=torch.bfloat16)
+    nv.attention_small(q, k, v, out, H, hd, scale)
+    report(f"attn_small L={L} H={H} hd={hd}", out, ref_of(), 1e-2, min_inside=0.999)
+    negative("attn_small (no rescale, 32-key tiles)", out, attn_ref_no_rescale(q, k, v, H, scale, hd=hd, tile=32), 1e-2, 0.999)
+    mask = (torch.rand(L, generator=g) > 0.3).to(torch.int32).to(dev)
+    out.fill_(float("nan"))
+    nv.attention_small(q, k, v, out, H, hd, scale, key_mask=mask)
+    report(f"attn_small L={L} key mask (30 % masked)", out, ref_of(mask), 1e-2, min_inside=0.999)
+    negative("attn_small key mask ignored", out, ref_of(), 1e-2, 0.999)
+    out.fill_(float("nan"))
+    nv.attention_small(q, k, v, out, H, hd, scale, key_mask=torch.zeros(L, dtype=torch.int32, device=dev))
+    ok = bool((out.float() == 0).all())
+    print(f"[{'OK ' if ok else 'BAD'}] attn_small every key masked: all outputs 0", flush=True)
+    RESULTS.append(("attn_small every key masked -> 0", ok))
+
+
 def sec_perf_gemm():
     g = torch.Generator(device="cpu").manual_seed(5)
     L = 32760
@@ -608,7 +862,10 @@ def _conv_runner():
     import torch.nn.functional as F
     g = torch.Generator(device="cpu").manual_seed(7)
 
-    def run(Cin, Cout, kt, kh, kw, T, H, W, pad, n_split=0, residual=False, fuse=None, variant=1, tag=""):
+    def run(Cin, Cout, kt, kh, kw, T, H, W, pad, n_split=0, residual=False, fuse=None, variant=1, tag="", tile_w=None):
+        """tile_w: None = 8 for W <= 8 else 16; "pick" = the VAE's _pick_tile_w(H, W); an int; or a list of widths run on
+        the same descriptor and inputs, whose outputs must be bit-identical (the per-pixel K loop does not depend on the
+        tile shape).  Returns the widths run."""
         S = T + 2
         xs = (torch.randn(S, H, W, Cin, generator=g) * 0.5)
         ring = torch.zeros(S + 1, H, W, Cin, dtype=torch.bfloat16, device=dev)
@@ -651,8 +908,6 @@ def _conv_runner():
             for t in range(T):
                 d.next_slot[t] = (t + 1) % (T + 2)
             d.next_gamma, d.next_silu, d.write_f32 = gamma.data_ptr(), 1, 1 if fuse == "both" else 0
-        nv.conv3d_causal(d)
-        torch.cuda.synchronize()
         xin = ring[:S].float().permute(3, 0, 1, 2).unsqueeze(0)        # [1,C,S,H,W]
         xin = xin[:, :, 3 - kt:] if kt < 3 else xin
         ref = F.conv3d(F.pad(xin, (pad, pad, pad, pad, 0, 0)) if kh == 3 else xin, w.to(dev).bfloat16().float(), b.to(dev))
@@ -661,20 +916,51 @@ def _conv_runner():
         ref = ref[0].permute(1, 2, 3, 0)[:T]                           # [T,H,W,Cout]
         if residual:
             ref = ref + res
+        want = F.silu(F.normalize(ref, dim=-1) * Cout ** 0.5 * gamma) if fuse is not None else None
         if n_split:
             ref = torch.stack([ref[..., :n_split], ref[..., n_split:]], dim=1).reshape(2 * T, H, W, n_split)
-        if fuse is not None:
-            want = F.silu(F.normalize(ref, dim=-1) * Cout ** 0.5 * gamma)
-            got = torch.stack([nring[(t + 1) % (T + 2)] for t in range(T)])
-            report(f"conv{tag} fused next-input ({fuse}) Cin={Cin} Cout={Cout} T={T} {H}x{W} res={residual}",
-                   got[..., :Cout].reshape(-1, Cout), want.reshape(-1, Cout), 2e-2)
-            report(f"conv{tag} fused next-input: padding channels and unused slots stay zero",
-                   torch.cat([got[..., Cout:].reshape(-1), nring[0].reshape(-1)]).unsqueeze(0) + 1,
-                   torch.ones(1, got[..., Cout:].numel() + nring[0].numel(), device=dev), 1e-7)
-            if fuse != "both":
-                return
-        report(f"conv{tag} Cin={Cin} Cout={Cout} k=({kt},{kh},{kw}) T={T} {H}x{W} split={n_split} res={residual}",
-               out.reshape(-1, out.shape[-1]), ref.reshape(-1, ref.shape[-1]), 2e-2)
+        if tile_w is None:
+            widths = [8 if W <= 8 else 16]
+        elif tile_w == "pick":
+            from diffsynth.models.wan_video_vae import _pick_tile_w
+            widths = [_pick_tile_w(H, W)]
+        else:
+            widths = [tile_w] if isinstance(tile_w, int) else list(tile_w)
+        first = None
+        for tw in widths:
+            d.tile_w = tw
+            out.fill_(float("nan"))
+            if fuse is not None:
+                nring.zero_()
+            nv.conv3d_causal(d)
+            torch.cuda.synchronize()
+            wtag = f"{tag} tile_w={tw}" if tile_w is not None else tag
+            if fuse is not None:
+                got = torch.stack([nring[(t + 1) % (T + 2)] for t in range(T)])
+                report(f"conv{wtag} fused next-input ({fuse}) Cin={Cin} Cout={Cout} T={T} {H}x{W} res={residual}",
+                       got[..., :Cout].reshape(-1, Cout), want.reshape(-1, Cout), 2e-2)
+                report(f"conv{wtag} fused next-input: padding channels and unused slots stay zero",
+                       torch.cat([got[..., Cout:].reshape(-1), nring[0].reshape(-1)]).unsqueeze(0) + 1,
+                       torch.ones(1, got[..., Cout:].numel() + nring[0].numel(), device=dev), 1e-7)
+            if fuse is None or fuse == "both":
+                report(f"conv{wtag} Cin={Cin} Cout={Cout} k=({kt},{kh},{kw}) T={T} {H}x{W} split={n_split} res={residual}",
+                       out.reshape(-1, out.shape[-1]), ref.reshape(-1, ref.shape[-1]), 2e-2)
+            outs = (out.clone(), nring.clone() if fuse is not None else None)
+            if first is None:
+                first = outs
+                if tile_w is not None:     # negative control: the reference shifted by one pixel along W fails the bar
+                    if fuse is None or fuse == "both":
+                        negative(f"conv{wtag} reference shifted by one pixel", out.reshape(-1, out.shape[-1]),
+                                 torch.roll(ref, 1, dims=-2).reshape(-1, ref.shape[-1]), 2e-2)
+                    else:
+                        negative(f"conv{wtag} fused next-input shifted by one pixel", got[..., :Cout].reshape(-1, Cout),
+                                 torch.roll(want, 1, dims=-2).reshape(-1, Cout), 2e-2)
+            else:
+                same = torch.equal(outs[0].nan_to_num(7.0), first[0].nan_to_num(7.0)) and \
+                    (fuse is None or torch.equal(outs[1], first[1]))
+                print(f"[{'OK ' if same else 'BAD'}] conv{tag} tile_w={tw} bit-identical to tile_w={widths[0]}", flush=True)
+                RESULTS.append((f"conv{tag} {H}x{W} tile_w={tw} bit-identical to tile_w={widths[0]}", same))
+        return widths
 
     return run
 
@@ -705,6 +991,29 @@ def sec_conv():
     run(384, 384, 3, 3, 3, 1, 2, 40, 1, residual=True)
     run(96, 4, 3, 3, 3, 2, 5, 200, 1)          # decoder head: 3 (+1) output channels on an N = 16 tile
     run(16, 48, 3, 3, 3, 1, 4, 140, 1, fuse="both")
+
+
+def sec_conv_tiles():
+    """Every tile width of svi_conv3d_causal (BW x BH = 8x16, 16x8, 32x4, 64x2, 128x1) on H and W that are not multiples of
+    the tile, with kt = 3 and 1, residual, the channel->frame split and the fused next input; the production geometries where
+    the VAE picks 32, 64 or 128; and each descriptor at all five widths with bit-identical outputs (measured so on an H100
+    80GB HBM3 at a 400 W power limit: fp32 output and fused bf16 next input identical for all six descriptors)."""
+    from diffsynth.models.wan_video_vae import _pick_tile_w
+    run = _conv_runner()
+    every = (8, 16, 32, 64, 128)
+    run(64, 96, 3, 3, 3, 2, 13, 150, 1, tile_w=every)
+    run(96, 96, 1, 3, 3, 1, 11, 70, 1, residual=True, tile_w=every)
+    run(384, 768, 3, 1, 1, 2, 6, 75, 0, n_split=384, tile_w=every)
+    run(96, 96, 3, 3, 3, 2, 9, 100, 1, fuse="only", tile_w=every)
+    run(192, 192, 3, 3, 3, 2, 7, 90, 1, residual=True, fuse="both", tile_w=every)
+    run(16, 48, 3, 3, 3, 1, 5, 19, 1, fuse="both", tile_w=every)
+    # where the VAE's tile choice is 32 (720p at 90x160 and 180x320), 64 (45-row band of a 320-wide stage) and 128 (45-row
+    # band of a 640-wide stage, 720p on 8 ranks)
+    for (H, W, want) in [(90, 160, 32), (180, 320, 32), (45, 320, 64), (45, 640, 128)]:
+        got = _pick_tile_w(H, W)
+        RESULTS.append((f"_pick_tile_w({H}, {W}) == {want}", got == want))
+        run(16, 32, 3, 3, 3, 1, H, W, 1, residual=True, tile_w="pick")
+    run(32, 16, 3, 3, 3, 2, 45, 640, 1, fuse="both", tile_w="pick")
 
 
 def sec_perf_conv():
