@@ -69,6 +69,12 @@ typedef struct svi_gemm_epilogue {
    * atomicAdd per group; the consumers (svi_rmsnorm_rope, svi_qk_norm_rope, svi_attn_fwd_qscale) add a group's partials in
    * index order, so a forward is bit-identical from run to run.  Needs sumsq_group_cols % 128 == 0.  0: atomicAdd. */
   int32_t sumsq_parts;
+  /* ---- weight format: 0 = W is bf16; 1 = W is float8_e4m3fn (ldw in elements = bytes), converted exactly to bf16 in shared
+   * memory ahead of the same bf16 wgmma, so the result is bit-identical to the bf16 GEMM on bf16(W) (weight-only FP8,
+   * vram_management/layers.py:65-71).  e4m3 needs K % 16 == 0 and ldw % 16 == 0 (16-byte TMA row pitch).
+   * Fields may be appended to this struct within one ABI version: callers must zero-initialise it (memset / `= {0}` /
+   * ctypes), so that a field they do not know about is 0 = today's behaviour. */
+  int32_t w_e4m3;
 } svi_gemm_epilogue;
 
 /*
@@ -77,7 +83,8 @@ typedef struct svi_gemm_epilogue {
  * Replaces every nn.Linear / F.linear on the path: wan_video_dit.py:227-229,242 (q,k,v,o),
  * :272-303 (cross-attn q,k,v,o,k_img,v_img), :334-335,372-373 (ffn.0/GELU/ffn.2 with gate+residual),
  * :401-404 (head), :429-452 (patch/text/time embeddings as GEMMs), vram_management/layers.py:65-71.
- * Requirements: K % 8 == 0, N % 8 == 0, lda % 8 == 0, ldw % 8 == 0, 16-byte aligned bases.
+ * Requirements: K % 8 == 0, N % 8 == 0, lda % 8 == 0, ldw % 8 == 0, 16-byte aligned bases; with ep->w_e4m3 = 1 (W e4m3)
+ * also K % 16 == 0 and ldw % 16 == 0.
  */
 int svi_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, int32_t M, int32_t N,
                   int32_t K, const svi_gemm_epilogue* ep, void* stream);

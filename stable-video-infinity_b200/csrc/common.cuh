@@ -40,10 +40,10 @@ void set_last_error(const char* fmt, ...);
     }                                                                                  \
   } while (0)
 
-// Encode a 2-D bf16 (or fp32) row-major tensor map with 128-byte swizzle. `inner` is the contiguous
-// dimension. Returns SVI_OK or an error code (message via set_last_error).
+// Encode a 2-D bf16 (or fp32, or 1-byte) row-major tensor map with 128-byte swizzle (or none: swizzle_128b = false).
+// `inner` is the contiguous dimension. Returns SVI_OK or an error code (message via set_last_error).
 int make_tmap_2d(CUtensorMap* map, const void* base, int elem_bytes, uint64_t inner, uint64_t outer,
-                 uint64_t row_pitch_bytes, uint32_t box_inner, uint32_t box_outer);
+                 uint64_t row_pitch_bytes, uint32_t box_inner, uint32_t box_outer, bool swizzle_128b = true);
 
 int sm_count();
 

@@ -4,6 +4,12 @@
 //   warpgroups 1, 2 : consumers, rows [0, 64) and [64, 128) of the 128 x 256 tile: wgmma m64n256k16 with the fp32
 //                     accumulator in registers, then the epilogue straight from those registers, 232 registers
 //
+// e4m3 weights (svi_gemm_epilogue.w_e4m3 = 1; the reference's weight-only FP8 mode): the producer lane TMA-loads the
+// 256 x 64 e4m3 W tile (16 KB, unswizzled) into a staging ring instead, and warps 1-3 of warpgroup 0 (idle in the bf16
+// instantiation) convert it, exactly, into the bf16 W tile in the same 128B-swizzled layout the bf16 TMA load produces.
+// The consumers, their wgmma descriptors and the epilogue are the same code, so the result is bit-identical to the bf16
+// GEMM on bf16(W).  Shared memory: 3 bf16 stages (144 KB) + 4 staging stages (64 KB) = 208 KB, against 4 x 48 KB for bf16.
+//
 // The producer runs ahead into the next tile while the consumers drain the previous one, so operand loads overlap the
 // epilogue.  Tiles are visited in groups of GROUP_M row blocks so that the CTAs resident together share A and W tiles in L2.
 // Replaces every F.linear of the reference's DiT (see include/svi_b200.h for the line map).
@@ -17,15 +23,63 @@ namespace gemm {
 constexpr int BM = 128;
 constexpr int BN = 256;
 constexpr int BK = 64;  // 64 bf16 = 128 B = one swizzle row
-constexpr int STAGES = 4;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
 constexpr int B_STAGE_BYTES = BN * BK * 2;  // 32 KB
 constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
+constexpr int W8_STAGE_BYTES = BN * BK;     // 16 KB of e4m3 W
 constexpr int NUM_THREADS = 384;
+constexpr int NUM_CONVERTERS = 96;          // warps 1-3 of warpgroup 0 (e4m3 instantiation)
 constexpr int GROUP_M = 8;
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 65536
 static_assert(A_STAGE_BYTES % 1024 == 0 && STAGE_BYTES % 1024 == 0, "operand tiles must stay 1024-byte aligned");
+
+// Ring depths per weight format: bf16 stages (A + bf16 W) and e4m3 staging stages.
+template <bool kE4M3> struct Rings;
+template <> struct Rings<false> { static constexpr int STAGES = 4, W8_STAGES = 0; };
+template <> struct Rings<true> { static constexpr int STAGES = 3, W8_STAGES = 4; };
+template <bool kE4M3>
+constexpr int smem_bytes() {
+  return Rings<kE4M3>::STAGES * STAGE_BYTES + Rings<kE4M3>::W8_STAGES * W8_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+}
+static_assert(smem_bytes<true>() <= 227 * 1024 && smem_bytes<false>() <= 227 * 1024, "shared memory over the sm_90 limit");
+
+// Four e4m3 codes (byte i = element i) -> bf16 elements 0,1 (.x) and 2,3 (.y), exactly.  Each code's sign goes to bit 15
+// and its 7 exponent|mantissa bits to bits 4..10 of a bf16, which reads as the e4m3 value times 2^-120 (the 4-bit
+// exponent field lands in the low bits of bf16's 8-bit one; code exponent 0 lands on bf16 subnormals, which is the e4m3
+// subnormal scale); one bf16x2 multiply by 2^120 is exact and restores the value, +-0 included.  The NaN codes 0x7F / 0xFF
+// (which would read as +-480) get their exponent and top mantissa bits set instead.
+__device__ __forceinline__ uint2 e4m3x4_to_bf16x4(uint32_t w) {
+  const uint32_t q = __byte_perm(w, 0, 0x3120);              // bytes [b0, b2, b1, b3]
+  const uint32_t q0 = q << 8;                                // halves hold b0 | b1 in their high bytes
+  uint32_t lo = (q0 & 0x80008000u) | ((q0 & 0x7F007F00u) >> 4);
+  uint32_t hi = (q & 0x80008000u) | ((q & 0x7F007F00u) >> 4); // b2 | b3
+  asm("mul.rn.bf16x2 %0, %0, %1;" : "+r"(lo) : "r"(0x7B807B80u));   // 2^120 in both halves
+  asm("mul.rn.bf16x2 %0, %0, %1;" : "+r"(hi) : "r"(0x7B807B80u));
+  const uint32_t nan = ((w & 0x7F7F7F7Fu) + 0x01010101u) & 0x80808080u;   // bit 7 of every byte whose code is +-NaN
+  if (nan) {
+    lo |= ((nan & 0x80u) ? 0x7FC0u : 0u) | ((nan & 0x8000u) ? 0x7FC00000u : 0u);
+    hi |= ((nan & 0x800000u) ? 0x7FC0u : 0u) | ((nan & 0x80000000u) ? 0x7FC00000u : 0u);
+  }
+  return make_uint2(lo, hi);
+}
+
+// One 256 x 64 e4m3 staging tile (row-major, 64 B per row) -> the bf16 W tile as the 128B-swizzled TMA load lays it out:
+// row r at byte 128 r, its 16-byte chunk j at chunk position j ^ (r & 7).  Thread t takes 16-byte source chunks t, t + 96, ...
+// (row i / 4, bf16 chunks 2 (i % 4) and 2 (i % 4) + 1); a quarter-warp's stores hit eight distinct bank groups.
+__device__ __forceinline__ void convert_w_tile(uint32_t src, uint32_t dst, int t) {
+#pragma unroll 2
+  for (int i = t; i < W8_STAGE_BYTES / 16; i += NUM_CONVERTERS) {
+    uint32_t w0, w1, w2, w3;
+    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(w0), "=r"(w1), "=r"(w2), "=r"(w3) : "r"(src + 16u * i));
+    const uint2 e0 = e4m3x4_to_bf16x4(w0), e1 = e4m3x4_to_bf16x4(w1), e2 = e4m3x4_to_bf16x4(w2), e3 = e4m3x4_to_bf16x4(w3);
+    const int r = i >> 2, j = 2 * (i & 3);
+    const uint32_t row = dst + 128u * r;
+    asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(row + 16u * (j ^ (r & 7))), "r"(e0.x), "r"(e0.y), "r"(e1.x),
+                 "r"(e1.y) : "memory");
+    asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(row + 16u * ((j + 1) ^ (r & 7))), "r"(e2.x), "r"(e2.y),
+                 "r"(e3.x), "r"(e3.y) : "memory");
+  }
+}
 
 struct Epi {
   void* out;
@@ -144,7 +198,7 @@ __device__ __forceinline__ void epilogue(const Epi& ep, float (&acc)[BN / 2], in
         }
         v0 += bv.x; v1 += bv.y;
         if (ep.act != SVI_ACT_NONE) apply_act2(v0, v1, ep.act);
-        ss[h] += v0 * v0 + v1 * v1;
+        ss[h] += fmaf(v0, v0, v1 * v1);   // contraction spelled out: identical in both weight-format instantiations
         v0 *= gv.x; v1 *= gv.y;
         if (ok[h]) {
           if (ep.residual) {
@@ -182,14 +236,19 @@ __device__ __forceinline__ void epilogue(const Epi& ep, float (&acc)[BN / 2], in
   }
 }
 
+template <bool kE4M3>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, int M, int N, int K,
                  const __grid_constant__ Epi ep) {
+  constexpr int STAGES = Rings<kE4M3>::STAGES, W8_STAGES = Rings<kE4M3>::W8_STAGES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bars = sbase + STAGES * STAGE_BYTES;
+  const uint32_t s8base = sbase + STAGES * STAGE_BYTES;          // e4m3 staging ring (e4m3 instantiation)
+  const uint32_t bars = s8base + W8_STAGES * W8_STAGE_BYTES;
   auto full_bar = [&](int s) { return bars + 8u * s; };
   auto empty_bar = [&](int s) { return bars + 8u * (STAGES + s); };
+  auto full8_bar = [&](int s) { return bars + 8u * (2 * STAGES + s); };               // staging tile landed
+  auto empty8_bar = [&](int s) { return bars + 8u * (2 * STAGES + W8_STAGES + s); };  // staging tile converted
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -203,8 +262,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     for (int i = 0; i < STAGES; ++i) {
-      mbar_init_a(full_bar(i), 1);
+      mbar_init_a(full_bar(i), kE4M3 ? 1 + NUM_CONVERTERS / 32 : 1);   // e4m3: + one arrive per converter warp
       mbar_init_a(empty_bar(i), 8);   // one arrive per consumer warp
+    }
+    for (int i = 0; i < W8_STAGES; ++i) {
+      mbar_init_a(full8_bar(i), 1);
+      mbar_init_a(empty8_bar(i), NUM_CONVERTERS / 32);
     }
     fence_mbar_init();
   }
@@ -214,18 +277,49 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     // ------------------------------- TMA producer -------------------------------
     setmaxnreg_dec<PRODUCER_REGS>();
     if (threadIdx.x == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      int stage = 0, stage8 = 0;
+      uint32_t phase = 0, phase8 = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         int m_blk, n_blk;
         tile_coords(tile, num_m, num_n, m_blk, n_blk);
         for (int kb = 0; kb < num_k; ++kb) {
           mbar_wait_a(empty_bar(stage), phase ^ 1);
-          mbar_expect_tx_a(full_bar(stage), STAGE_BYTES);
           const uint32_t sa = sbase + stage * STAGE_BYTES;
-          tma_load_2d_a(sa, &tmap_a, full_bar(stage), kb * BK, m_blk * BM);
-          tma_load_2d_a(sa + A_STAGE_BYTES, &tmap_b, full_bar(stage), kb * BK, n_blk * BN);
+          if constexpr (kE4M3) {
+            mbar_expect_tx_a(full_bar(stage), A_STAGE_BYTES);
+            tma_load_2d_a(sa, &tmap_a, full_bar(stage), kb * BK, m_blk * BM);
+            mbar_wait_a(empty8_bar(stage8), phase8 ^ 1);
+            mbar_expect_tx_a(full8_bar(stage8), W8_STAGE_BYTES);
+            tma_load_2d_a(s8base + stage8 * W8_STAGE_BYTES, &tmap_b, full8_bar(stage8), kb * BK, n_blk * BN);
+            if (++stage8 == W8_STAGES) { stage8 = 0; phase8 ^= 1; }
+          } else {
+            mbar_expect_tx_a(full_bar(stage), STAGE_BYTES);
+            tma_load_2d_a(sa, &tmap_a, full_bar(stage), kb * BK, m_blk * BM);
+            tma_load_2d_a(sa + A_STAGE_BYTES, &tmap_b, full_bar(stage), kb * BK, n_blk * BN);
+          }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    } else if (kE4M3 && warp >= 1) {
+      // ------------------------------- e4m3 -> bf16 W converters -------------------------------
+      // The staging tile of k-block i lands after the producer saw bf16 stage (i mod STAGES) freed by the consumers, so its
+      // W half may be written once full8 completes.  The writes are generic-proxy stores that wgmma (async proxy) reads:
+      // every writer fences before its warp's arrive on the stage's full barrier.
+      const int t = threadIdx.x - 32;
+      int stage = 0, stage8 = 0;
+      uint32_t phase8 = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        for (int kb = 0; kb < num_k; ++kb) {
+          mbar_wait_a(full8_bar(stage8), phase8);
+          convert_w_tile(s8base + stage8 * W8_STAGE_BYTES, sbase + stage * STAGE_BYTES + A_STAGE_BYTES, t);
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+          __syncwarp();
+          if (lane == 0) {
+            mbar_arrive_a(empty8_bar(stage8));
+            mbar_arrive_a(full_bar(stage));
+          }
+          if (++stage8 == W8_STAGES) { stage8 = 0; phase8 ^= 1; }
+          if (++stage == STAGES) stage = 0;
         }
       }
     }
@@ -263,6 +357,28 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   }
 }
 
+// Sets the dynamic shared-memory size of one instantiation once per process, then launches it.
+template <bool kE4M3>
+int launch(const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, const Epi& ep, cudaStream_t stream) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t ce = cudaFuncSetAttribute(gemm_bf16_kernel<kE4M3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          smem_bytes<kE4M3>());
+    if (ce != cudaSuccess) {
+      set_last_error("svi_gemm_bf16: cudaFuncSetAttribute failed: %s", cudaGetErrorString(ce));
+      return SVI_ERR_LAUNCH;
+    }
+    attr_set = true;
+  }
+  const int num_tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
+  const int sms = sm_count();
+  if (sms <= 0) return SVI_ERR_DRIVER;
+  const int grid = num_tiles < sms ? num_tiles : sms;
+  gemm_bf16_kernel<kE4M3><<<grid, NUM_THREADS, smem_bytes<kE4M3>(), stream>>>(ta, tb, M, N, K, ep);
+  SVI_CUDA_LAUNCH_CHECK("svi_gemm_bf16");
+  return SVI_OK;
+}
+
 }  // namespace gemm
 }  // namespace svi
 
@@ -275,6 +391,11 @@ extern "C" int svi_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t 
   SVI_REQUIRE(K % 8 == 0 && N % 8 == 0, "svi_gemm_bf16: K and N must be multiples of 8 (K=%d N=%d)", K, N);
   SVI_REQUIRE(lda % 8 == 0 && ldw % 8 == 0 && lda >= K && ldw >= K,
               "svi_gemm_bf16: lda/ldw must be multiples of 8 and >= K");
+  SVI_REQUIRE(e->w_e4m3 == 0 || e->w_e4m3 == 1, "svi_gemm_bf16: w_e4m3 must be 0 (bf16 W) or 1 (e4m3 W), got %d", e->w_e4m3);
+  if (e->w_e4m3)
+    SVI_REQUIRE(K % 16 == 0 && ldw % 16 == 0,
+                "svi_gemm_bf16: e4m3 W needs K and ldw to be multiples of 16 (16-byte row pitch; K=%d ldw=%lld)", K,
+                (long long)ldw);
   SVI_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(W) & 15) == 0,
               "svi_gemm_bf16: A and W must be 16-byte aligned");
   SVI_REQUIRE(e->ldo >= N && e->ldo % (e->out_is_f32 ? 4 : 8) == 0 &&
@@ -304,7 +425,10 @@ extern "C" int svi_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t 
   CUtensorMap ta, tb;
   int rc = make_tmap_2d(&ta, A, 2, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, BK, BM);
   if (rc) return rc;
-  rc = make_tmap_2d(&tb, W, 2, (uint64_t)K, (uint64_t)N, (uint64_t)ldw * 2, BK, BN);
+  if (e->w_e4m3)   // the converters swizzle; the staging tile is plain 64-byte rows
+    rc = make_tmap_2d(&tb, W, 1, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, BK, BN, /*swizzle_128b=*/false);
+  else
+    rc = make_tmap_2d(&tb, W, 2, (uint64_t)K, (uint64_t)N, (uint64_t)ldw * 2, BK, BN);
   if (rc) return rc;
 
   Epi ep;
@@ -314,20 +438,6 @@ extern "C" int svi_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t 
   ep.ln_stats = e->ln_stats; ep.ln_u = e->ln_u; ep.ln_inv_d = e->ln_dim > 0 ? 1.0f / (float)e->ln_dim : 0.f; ep.ln_eps = e->ln_eps;
   ep.a_next = reinterpret_cast<__nv_bfloat16*>(e->a_next); ep.ld_an = e->ld_an; ep.g_next = e->g_next; ep.row_stats = e->row_stats;
 
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t ce = cudaFuncSetAttribute(gemm_bf16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (ce != cudaSuccess) {
-      set_last_error("svi_gemm_bf16: cudaFuncSetAttribute failed: %s", cudaGetErrorString(ce));
-      return SVI_ERR_LAUNCH;
-    }
-    attr_set = true;
-  }
-  const int num_tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
-  const int sms = sm_count();
-  if (sms <= 0) return SVI_ERR_DRIVER;
-  const int grid = num_tiles < sms ? num_tiles : sms;
-  gemm_bf16_kernel<<<grid, NUM_THREADS, SMEM_BYTES, static_cast<cudaStream_t>(stream)>>>(ta, tb, M, N, K, ep);
-  SVI_CUDA_LAUNCH_CHECK("svi_gemm_bf16");
-  return SVI_OK;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return e->w_e4m3 ? launch<true>(ta, tb, M, N, K, ep, st) : launch<false>(ta, tb, M, N, K, ep, st);
 }

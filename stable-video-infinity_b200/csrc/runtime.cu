@@ -38,15 +38,17 @@ static EncodeTiledFn get_encode_fn() {
 }
 
 int make_tmap_2d(CUtensorMap* map, const void* base, int elem_bytes, uint64_t inner, uint64_t outer,
-                 uint64_t row_pitch_bytes, uint32_t box_inner, uint32_t box_outer) {
+                 uint64_t row_pitch_bytes, uint32_t box_inner, uint32_t box_outer, bool swizzle_128b) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return SVI_ERR_DRIVER;
   CUtensorMapDataType dt;
   if (elem_bytes == 2) dt = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   else if (elem_bytes == 4) dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  else if (elem_bytes == 1) dt = CU_TENSOR_MAP_DATA_TYPE_UINT8;
   else { set_last_error("make_tmap_2d: unsupported element size %d", elem_bytes); return SVI_ERR_INVALID_ARG; }
   if (box_inner * (uint32_t)elem_bytes > 128 || box_outer > 256) {
-    set_last_error("make_tmap_2d: box %ux%u too large for 128B swizzle", box_inner, box_outer);
+    set_last_error("make_tmap_2d: box %ux%u too large (inner box at most 128 bytes, outer at most 256 rows)", box_inner,
+                   box_outer);
     return SVI_ERR_INVALID_ARG;
   }
   cuuint64_t dims[2] = {inner, outer};
@@ -54,7 +56,7 @@ int make_tmap_2d(CUtensorMap* map, const void* base, int elem_bytes, uint64_t in
   cuuint32_t box[2] = {box_inner, box_outer};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(map, dt, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_128b ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_last_error("cuTensorMapEncodeTiled failed (CUresult %d): base=%p inner=%llu outer=%llu pitch=%llu box=%ux%u",

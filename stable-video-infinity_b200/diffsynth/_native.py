@@ -26,7 +26,7 @@ class GemmEpilogue(_c.Structure):
         ("sumsq", _vp), ("sumsq_groups", _i32), ("sumsq_group_cols", _i32),
         ("ln_stats", _vp), ("ln_u", _vp), ("ln_dim", _i32), ("ln_eps", _f32),
         ("a_next", _vp), ("ld_an", _i64), ("g_next", _vp), ("row_stats", _vp),
-        ("sumsq_parts", _i32),
+        ("sumsq_parts", _i32), ("w_e4m3", _i32),
     ]
 
 
@@ -168,15 +168,28 @@ def sm_count():
 
 
 def gemm(a, w, out, bias=None, act=ACT_NONE, gate=None, residual=None, sumsq=None, sumsq_group_cols=0, ln=None, emit=None):
-    """out = epilogue(a[M,K] @ w[N,K]^T); a, w bf16; out f32 or bf16 (may be a column slice view).
+    """out = epilogue(a[M,K] @ w[N,K]^T); a bf16, w bf16 or float8_e4m3fn; out f32 or bf16 (may be a column slice view).
+    An e4m3 w is converted exactly to bf16 inside the kernel (weight-only FP8): the result is bit-identical to passing
+    w.to(torch.bfloat16); it needs K % 16 == 0 and a row stride that is a multiple of 16.
     ln = (stats f32 [M,2], u f32 [N], dim, eps): LayerNorm folded into the GEMM (consumer side, svi_gemm_epilogue);
     emit = (a_next bf16 [M,N], g_next f32 [N], row_stats f32 [M,2]): producer side."""
+    if a.dtype != torch.bfloat16:
+        raise RuntimeError(f"svi_b200.gemm: a must be bf16 (only the weight may be float8_e4m3fn), got {a.dtype}")
+    if w.dtype not in (torch.bfloat16, torch.float8_e4m3fn):
+        raise RuntimeError(f"svi_b200.gemm: w must be bf16 or float8_e4m3fn (e5m2 and other formats are not supported), "
+                           f"got {w.dtype}")
+    if emit is not None and emit[0].dtype != torch.bfloat16:
+        raise RuntimeError(f"svi_b200.gemm: emit's a_next must be bf16, got {emit[0].dtype}")
     lda, ldw, ldo = _rowmajor(a, "a"), _rowmajor(w, "w"), _rowmajor(out, "out")
     M, K = a.shape
     N = w.shape[0]
     if w.shape[1] != K or out.shape[0] != M or out.shape[1] != N:
         raise RuntimeError(f"svi_b200.gemm: shape mismatch a{tuple(a.shape)} w{tuple(w.shape)} out{tuple(out.shape)}")
+    w_e4m3 = w.dtype == torch.float8_e4m3fn
+    if w_e4m3 and (K % 16 or ldw % 16):
+        raise RuntimeError(f"svi_b200.gemm: an e4m3 w needs K and its row stride to be multiples of 16 (K={K}, stride={ldw})")
     ep = GemmEpilogue()
+    ep.w_e4m3 = int(w_e4m3)
     ep.out = _ptr(out, name="out")
     ep.ldo = ldo
     if out.dtype == torch.float32:
@@ -213,7 +226,7 @@ def gemm(a, w, out, bias=None, act=ACT_NONE, gate=None, residual=None, sumsq=Non
             raise RuntimeError("svi_b200.gemm: emit needs a_next [M,N] and contiguous row_stats [M,2]")
         ep.a_next, ep.ld_an = _ptr(a_next, torch.bfloat16, "a_next"), _rowmajor(a_next, "a_next")
         ep.g_next, ep.row_stats = _ptr(g_next, torch.float32, "g_next"), _ptr(row_stats, torch.float32, "row_stats")
-    rc = load().svi_gemm_bf16(_ptr(a, torch.bfloat16, "a"), lda, _ptr(w, torch.bfloat16, "w"), ldw,
+    rc = load().svi_gemm_bf16(_ptr(a, torch.bfloat16, "a"), lda, _ptr(w, name="w"), ldw,
                               M, N, K, ctypes.byref(ep), _stream())
     _check(rc, "svi_gemm_bf16")
     return out

@@ -157,38 +157,47 @@ def _bf16(t, device):
     return t.detach().to(device=device, dtype=torch.bfloat16).contiguous()
 
 
+def _mat(t, device):
+    """Kernel-ready GEMM weight.  A model loaded as float8_e4m3fn (the reference's weight-only FP8 mode) keeps its matrices
+    e4m3 on the device: svi_gemm_bf16 converts them exactly to bf16 in shared memory, so the result is the same as from the
+    upcast copy at half the bytes.  A matrix whose K is not a multiple of 16 (the e4m3 TMA row pitch) is upcast to bf16."""
+    if t.dtype == torch.float8_e4m3fn and t.shape[-1] % 16 == 0:
+        return t.detach().to(device=device).contiguous()
+    return _bf16(t, device)
+
+
 class _BlockWeights:
     """Kernel-ready copies of one DiTBlock's parameters (fused QKV / KV weights, fp32 vectors)."""
 
     def __init__(self, blk: DiTBlock, device):
         sa, ca = blk.self_attn, blk.cross_attn
-        self.w_qkv = _bf16(torch.cat([sa.q.weight, sa.k.weight, sa.v.weight], 0), device)
+        self.w_qkv = _mat(torch.cat([sa.q.weight, sa.k.weight, sa.v.weight], 0), device)
         self.b_qkv = _f32(torch.cat([sa.q.bias, sa.k.bias, sa.v.bias], 0), device)
         self.w_q, self.b_q = self.w_qkv[: blk.dim], self.b_qkv[: blk.dim]          # views (sequence-parallel split)
         self.w_kv, self.b_kv = self.w_qkv[blk.dim:], self.b_qkv[blk.dim:]
-        self.w_o, self.b_o = _bf16(sa.o.weight, device), _f32(sa.o.bias, device)
+        self.w_o, self.b_o = _mat(sa.o.weight, device), _f32(sa.o.bias, device)
         self.nq, self.nk = _f32(sa.norm_q.weight, device), _f32(sa.norm_k.weight, device)
         self.eps_qk = sa.norm_q.eps
-        self.w_cq, self.b_cq = _bf16(ca.q.weight, device), _f32(ca.q.bias, device)
-        self.w_ckv = _bf16(torch.cat([ca.k.weight, ca.v.weight], 0), device)
+        self.w_cq, self.b_cq = _mat(ca.q.weight, device), _f32(ca.q.bias, device)
+        self.w_ckv = _mat(torch.cat([ca.k.weight, ca.v.weight], 0), device)
         self.b_ckv = _f32(torch.cat([ca.k.bias, ca.v.bias], 0), device)
-        self.w_co, self.b_co = _bf16(ca.o.weight, device), _f32(ca.o.bias, device)
+        self.w_co, self.b_co = _mat(ca.o.weight, device), _f32(ca.o.bias, device)
         # cross-attention q is never normalised in memory: its RMS factor rides in the attention's softmax scale
         # (svi_attn_fwd_qscale) and norm_q's channel weight is folded into the (step-invariant) K:  q.w_q . k = q . (w_q k)
         self.cnk_q = _f32(ca.norm_k.weight.detach().float() * ca.norm_q.weight.detach().float(), device)
         if ca.has_image_input:
-            self.w_ckv_img = _bf16(torch.cat([ca.k_img.weight, ca.v_img.weight], 0), device)
+            self.w_ckv_img = _mat(torch.cat([ca.k_img.weight, ca.v_img.weight], 0), device)
             self.b_ckv_img = _f32(torch.cat([ca.k_img.bias, ca.v_img.bias], 0), device)
             self.cnk_img_q = _f32(ca.norm_k_img.weight.detach().float() * ca.norm_q.weight.detach().float(), device)
         self.n3w, self.n3b = _f32(blk.norm3.weight, device), _f32(blk.norm3.bias, device)
         self.eps = blk.norm1.eps
-        self.w_f0, self.b_f0 = _bf16(blk.ffn[0].weight, device), _f32(blk.ffn[0].bias, device)
-        self.w_f2, self.b_f2 = _bf16(blk.ffn[2].weight, device), _f32(blk.ffn[2].bias, device)
+        self.w_f0, self.b_f0 = _mat(blk.ffn[0].weight, device), _f32(blk.ffn[0].bias, device)
+        self.w_f2, self.b_f2 = _mat(blk.ffn[2].weight, device), _f32(blk.ffn[2].bias, device)
         if getattr(blk, "enable_multitalk", False):
             a = blk.audio_cross_attn
-            self.w_aq, self.b_aq = _bf16(a.q_linear.weight, device), _f32(a.q_linear.bias, device)
-            self.w_akv, self.b_akv = _bf16(a.kv_linear.weight, device), _f32(a.kv_linear.bias, device)
-            self.w_ap, self.b_ap = _bf16(a.proj.weight, device), _f32(a.proj.bias, device)
+            self.w_aq, self.b_aq = _mat(a.q_linear.weight, device), _f32(a.q_linear.bias, device)
+            self.w_akv, self.b_akv = _mat(a.kv_linear.weight, device), _f32(a.kv_linear.bias, device)
+            self.w_ap, self.b_ap = _mat(a.proj.weight, device), _f32(a.proj.bias, device)
             self.nxw, self.nxb = _f32(blk.norm_x.weight, device), _f32(blk.norm_x.bias, device)
 
 
@@ -302,29 +311,29 @@ class WanDiTEngine:
         self.blocks = [_BlockWeights(b, self.device) for b in model.blocks]
         pe = model.patch_embedding
         self.kpatch = pe.weight.shape[1] * 4
-        self.w_patch = _bf16(pe.weight.reshape(d, self.kpatch), self.device)
+        self.w_patch = _mat(pe.weight.reshape(d, self.kpatch), self.device)
         self.b_patch = _f32(pe.bias, self.device)
-        self.w_te0, self.b_te0 = _bf16(model.text_embedding[0].weight, self.device), _f32(model.text_embedding[0].bias, self.device)
-        self.w_te2, self.b_te2 = _bf16(model.text_embedding[2].weight, self.device), _f32(model.text_embedding[2].bias, self.device)
-        self.w_t0, self.b_t0 = _bf16(model.time_embedding[0].weight, self.device), _f32(model.time_embedding[0].bias, self.device)
-        self.w_t2, self.b_t2 = _bf16(model.time_embedding[2].weight, self.device), _f32(model.time_embedding[2].bias, self.device)
-        self.w_tp, self.b_tp = _bf16(model.time_projection[1].weight, self.device), _f32(model.time_projection[1].bias, self.device)
-        self.w_head, self.b_head = _bf16(model.head.head.weight, self.device), _f32(model.head.head.bias, self.device)
+        self.w_te0, self.b_te0 = _mat(model.text_embedding[0].weight, self.device), _f32(model.text_embedding[0].bias, self.device)
+        self.w_te2, self.b_te2 = _mat(model.text_embedding[2].weight, self.device), _f32(model.text_embedding[2].bias, self.device)
+        self.w_t0, self.b_t0 = _mat(model.time_embedding[0].weight, self.device), _f32(model.time_embedding[0].bias, self.device)
+        self.w_t2, self.b_t2 = _mat(model.time_embedding[2].weight, self.device), _f32(model.time_embedding[2].bias, self.device)
+        self.w_tp, self.b_tp = _mat(model.time_projection[1].weight, self.device), _f32(model.time_projection[1].bias, self.device)
+        self.w_head, self.b_head = _mat(model.head.head.weight, self.device), _f32(model.head.head.bias, self.device)
         self.head_mod = _f32(model.head.modulation.reshape(2, d), self.device)
         self.mod_table = _f32(torch.cat([b.modulation.reshape(6, d) for b in model.blocks], 0), self.device)   # [6*layers, d]
         self.eps = model.head.norm.eps
         if model.has_image_input:
             p = model.img_emb.proj
             self.ie_ln0 = (_f32(p[0].weight, self.device), _f32(p[0].bias, self.device), p[0].eps)
-            self.ie_w1, self.ie_b1 = _bf16(p[1].weight, self.device), _f32(p[1].bias, self.device)
-            self.ie_w3, self.ie_b3 = _bf16(p[3].weight, self.device), _f32(p[3].bias, self.device)
+            self.ie_w1, self.ie_b1 = _mat(p[1].weight, self.device), _f32(p[1].bias, self.device)
+            self.ie_w3, self.ie_b3 = _mat(p[3].weight, self.device), _f32(p[3].bias, self.device)
             self.ie_ln4 = (_f32(p[4].weight, self.device), _f32(p[4].bias, self.device), p[4].eps)
         if getattr(model, "enable_multitalk", False):
             ap = model.audio_proj
-            self.ap_w1, self.ap_b1 = _bf16(ap.proj1.weight, self.device), _f32(ap.proj1.bias, self.device)
-            self.ap_w1v, self.ap_b1v = _bf16(ap.proj1_vf.weight, self.device), _f32(ap.proj1_vf.bias, self.device)
-            self.ap_w2, self.ap_b2 = _bf16(ap.proj2.weight, self.device), _f32(ap.proj2.bias, self.device)
-            self.ap_w3, self.ap_b3 = _bf16(ap.proj3.weight, self.device), _f32(ap.proj3.bias, self.device)
+            self.ap_w1, self.ap_b1 = _mat(ap.proj1.weight, self.device), _f32(ap.proj1.bias, self.device)
+            self.ap_w1v, self.ap_b1v = _mat(ap.proj1_vf.weight, self.device), _f32(ap.proj1_vf.bias, self.device)
+            self.ap_w2, self.ap_b2 = _mat(ap.proj2.weight, self.device), _f32(ap.proj2.bias, self.device)
+            self.ap_w3, self.ap_b3 = _mat(ap.proj3.weight, self.device), _f32(ap.proj3.bias, self.device)
             self.ap_ln = (_f32(ap.norm.weight, self.device), _f32(ap.norm.bias, self.device), ap.norm.eps)
             self.ap_tokens, self.ap_dim = ap.context_tokens, ap.output_dim
         self._rope = {}

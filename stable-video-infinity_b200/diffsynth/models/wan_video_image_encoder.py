@@ -148,11 +148,13 @@ class WanImageEncoder(nn.Module):
         return self._engine[1]
 
     def encode_image(self, videos):
-        """list of f32 [1,3,H,W] images in [-1,1] -> [B, 257, 1280] in the parameter dtype (reference :864-880)."""
+        """list of f32 [1,3,H,W] images in [-1,1] -> [B, 257, 1280] in the parameter dtype (bf16 for float8 parameters,
+        see wan_video_text_encoder.output_dtype) (reference :864-880)."""
+        from .wan_video_text_encoder import output_dtype
         p = self.model.visual.patch_embedding.weight
         eng = self.engine(p.device)
         outs = [eng.forward(eng.preprocess(u)) for u in videos]
-        return torch.cat(outs, dim=0).to(p.dtype)
+        return torch.cat(outs, dim=0).to(output_dtype(p.dtype))
 
     @staticmethod
     def state_dict_converter():

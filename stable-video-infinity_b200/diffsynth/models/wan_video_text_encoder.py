@@ -78,6 +78,12 @@ def relative_position_buckets(lq, lk, num_buckets=32, max_dist=128):
     return (side + torch.where(dist < exact, dist, log_bin)).to(torch.int32)
 
 
+def output_dtype(param_dtype):
+    """Dtype an encoder returns for parameters of `param_dtype`: the parameter dtype, except that float8 parameters are
+    weight-only storage whose compute dtype is bf16 (reference vram_management/layers.py:65-71, computation_dtype)."""
+    return torch.bfloat16 if param_dtype in (torch.float8_e4m3fn, torch.float8_e5m2) else param_dtype
+
+
 class WanTextEncoderEngine:
     """Kernel-ready weights of one WanTextEncoder on one device + the forward that drives the native kernels."""
 
@@ -89,7 +95,12 @@ class WanTextEncoderEngine:
         self.num_buckets = model.num_buckets
         bf = lambda t: t.detach().to(device=self.device, dtype=torch.bfloat16).contiguous()
         f32 = lambda t: t.detach().to(device=self.device, dtype=torch.float32).contiguous()
-        self.table = bf(model.token_embedding.weight)
+
+        def mat(t):   # GEMM weight: a model loaded as float8_e4m3fn stays e4m3 (svi_gemm_bf16 converts it exactly)
+            if t.dtype == torch.float8_e4m3fn and t.shape[-1] % 16 == 0:
+                return t.detach().to(device=self.device).contiguous()
+            return bf(t)
+        self.table = bf(model.token_embedding.weight)     # stays bf16: svi_embedding_gather reads bf16 rows
         self.norm_w, self.eps = f32(model.norm.weight), model.norm.eps
         if model.shared_pos:
             raise NotImplementedError("shared_pos=True (T5 v1.0 style single bias table) is not used by umT5 / Wan")
@@ -97,8 +108,8 @@ class WanTextEncoderEngine:
         for b in model.blocks:
             self.layers.append(dict(
                 n1=f32(b.norm1.weight), n2=f32(b.norm2.weight), eps=b.norm1.eps,
-                w_qkv=bf(torch.cat([b.attn.q.weight, b.attn.k.weight, b.attn.v.weight], 0)), w_o=bf(b.attn.o.weight),
-                w_gate=bf(b.ffn.gate[0].weight), w_fc1=bf(b.ffn.fc1.weight), w_fc2=bf(b.ffn.fc2.weight),
+                w_qkv=mat(torch.cat([b.attn.q.weight, b.attn.k.weight, b.attn.v.weight], 0)), w_o=mat(b.attn.o.weight),
+                w_gate=mat(b.ffn.gate[0].weight), w_fc1=mat(b.ffn.fc1.weight), w_fc2=mat(b.ffn.fc2.weight),
                 bias=f32(b.pos_embedding.embedding.weight)))          # [num_buckets, H]
         self._buckets = {}
         self.launches = 0
@@ -170,10 +181,11 @@ class WanTextEncoder(nn.Module):
         return self._engine[1]
 
     def forward(self, ids, mask=None):
-        """[1, L] token ids (+ padding mask) -> [1, L, dim] in the parameter dtype."""
+        """[1, L] token ids (+ padding mask) -> [1, L, dim] in the parameter dtype; bf16 for float8 parameters, which hold
+        weights only (the reference's FP8 mode computes the encoder in bf16 and returns bf16)."""
         dev = ids.device if ids.is_cuda else self.token_embedding.weight.device
         out = self.engine(dev).forward(ids, mask)
-        return out.to(self.token_embedding.weight.dtype)
+        return out.to(output_dtype(self.token_embedding.weight.dtype))
 
     @staticmethod
     def state_dict_converter():
