@@ -268,7 +268,13 @@ int svi_axpby(const float* a, float alpha, const float* b, float beta, float* ou
  * Weights: bf16 [w_rows, w_ld], row = output channel, column = ((a*kh + b)*kw + c)*ceil64(C_in) + channel.
  * Output: f32 channels-last, frame t at out + t*out_frame_stride, pixel pitch out_ld; columns >= n_split
  * (if n_split > 0) go to out + split_offset with column - n_split (upsample3d channel->frame split :153-156).
- * out = conv + bias (+ residual).
+ * out = conv + bias (+ residual); bias == NULL adds zero.
+ * The epilogue moves channel pairs (float2 / bf16x2), so it requires: C_out, out_ld, next_ld % 4 == 0; n_split,
+ * split_offset, out_frame_stride, res_ld, res_frame_stride and next_frame_stride even; out, bias, residual and next_gamma
+ * 8-byte aligned, next_ring 4-byte aligned, x_ring and w_packed 16-byte aligned (TMA); out_ld >= C_out without a split and
+ * out_ld >= max(n_split, C_out - n_split) with one (checked only when the fp32 output is written); res_ld >= C_out.
+ * Packed-weight columns of channels >= C_in are multiplied by zero (the ring is read with zero fill) and may hold anything
+ * finite.
  */
 typedef struct svi_conv_desc {
   const void* x_ring; int32_t ring_slots, in_H, in_W, C_in;

@@ -314,6 +314,38 @@ extern "C" int svi_conv3d_causal(const svi_conv_desc* d, void* stream) {
   for (int w : kWidths)
     if (w >= BN) { BN = w; break; }
   SVI_REQUIRE(d->w_rows >= d->C_out, "svi_conv3d_causal: packed weight has fewer rows than C_out");
+  // The epilogue moves channel pairs (n, n + 1), n even: float2 loads of bias / residual / next_gamma, float2 stores to out
+  // and bf16x2 stores to next_ring.  Every offset added to n must therefore be even and every base aligned to the pair.
+  const bool writes_out = !d->next_ring || d->write_f32;
+  SVI_REQUIRE(d->n_split % 2 == 0, "svi_conv3d_causal: n_split must be even (got %d)", d->n_split);
+  if (writes_out) {
+    SVI_REQUIRE((reinterpret_cast<uintptr_t>(d->out) & 7) == 0, "svi_conv3d_causal: out must be 8-byte aligned");
+    SVI_REQUIRE(d->out_frame_stride % 2 == 0, "svi_conv3d_causal: out_frame_stride must be even (got %lld)",
+                (long long)d->out_frame_stride);
+    if (d->n_split > 0) {
+      SVI_REQUIRE(d->split_offset % 2 == 0, "svi_conv3d_causal: split_offset must be even (got %lld)",
+                  (long long)d->split_offset);
+      SVI_REQUIRE(d->out_ld >= d->n_split && d->out_ld >= d->C_out - d->n_split,
+                  "svi_conv3d_causal: out_ld must be >= max(n_split, C_out - n_split) (got out_ld %d)", d->out_ld);
+    } else {
+      SVI_REQUIRE(d->out_ld >= d->C_out, "svi_conv3d_causal: out_ld must be >= C_out (got out_ld %d, C_out %d)", d->out_ld,
+                  d->C_out);
+    }
+  }
+  SVI_REQUIRE((reinterpret_cast<uintptr_t>(d->bias) & 7) == 0, "svi_conv3d_causal: bias must be 8-byte aligned");
+  if (d->residual) {
+    SVI_REQUIRE((reinterpret_cast<uintptr_t>(d->residual) & 7) == 0, "svi_conv3d_causal: residual must be 8-byte aligned");
+    SVI_REQUIRE(d->res_ld >= d->C_out && d->res_ld % 2 == 0, "svi_conv3d_causal: res_ld must be even and >= C_out (got %d)",
+                d->res_ld);
+    SVI_REQUIRE(d->res_frame_stride % 2 == 0, "svi_conv3d_causal: res_frame_stride must be even (got %lld)",
+                (long long)d->res_frame_stride);
+  }
+  if (d->next_ring) {
+    SVI_REQUIRE((reinterpret_cast<uintptr_t>(d->next_ring) & 3) == 0, "svi_conv3d_causal: next_ring must be 4-byte aligned");
+    SVI_REQUIRE(d->next_frame_stride % 2 == 0, "svi_conv3d_causal: next_frame_stride must be even (got %lld)",
+                (long long)d->next_frame_stride);
+    SVI_REQUIRE((reinterpret_cast<uintptr_t>(d->next_gamma) & 7) == 0, "svi_conv3d_causal: next_gamma must be 8-byte aligned");
+  }
   // variant: kept in the descriptor so that callers of the C ABI stay valid; every value runs the one kernel of this file
   SVI_REQUIRE(d->variant >= 0 && d->variant <= 2, "svi_conv3d_causal: variant must be 0 (auto), 1 or 2");
   SVI_REQUIRE(d->variant != 2 || (d->kw == 3 && d->pad_w == 1), "svi_conv3d_causal: variant 2 needs k_w = 3 and pad_w = 1");
