@@ -97,7 +97,13 @@ int svi_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, int32_
  * workspace (optional, 16-byte aligned device memory of workspace_bytes, may be NULL / 0): lets the launch cut the
  * (head, Q-tile) units of its last, partly filled wave of CTAs into K/V slices that are merged by a second
  * kernel (log-sum-exp merge), so all SMs stay busy; svi_attn_workspace_bytes() returns the size that allows every
- * plan.  The library never allocates.  Results are the same function of the inputs either way (fp32 merge).
+ * plan.  The library never allocates; a launch touches only the first slices * 66560 bytes of the workspace its plan
+ * (svi_attn_plan) uses.  What holds: every plan is within the same fp64 error bound of softmax(Q K^T * scale) V
+ * (about 2^-8 of sum_j softmax_j |v_j| per element, from the bf16 P); a given plan is bit-reproducible and within one
+ * bf16 ulp, plus a floor of fp32 rounding, of its own kernel-order result.  Different plans are NOT interchangeable bit
+ * for bit: each K/V slice rounds its bf16 P against its own running row max, so on the units a plan slices another plan
+ * (with or without a workspace, or the SP visit order) can change a large share of the outputs, some by more than one
+ * bf16 ulp (outputs near zero by many).  Compare results of different plans with the fp64 bound, not with a ulp count.
  * Replaces flash_attention(), wan_video_dit.py:116-147 (the single attention entry point).
  */
 int svi_attn_fwd(const void* Q, int64_t ldq, const void* K, int64_t ldk, const void* V, int64_t ldv,
@@ -108,8 +114,8 @@ size_t svi_attn_workspace_bytes(int32_t Lq, int32_t Lk, int32_t num_heads);
  * svi_attn_fwd with the full-width RMSNorm of Q folded into the softmax scale: row r of Q is used as
  * Q[r,:] * rsqrt(S_r / q_dim + q_eps), S_r = q_sumsq[r * q_ss_ld] (q_ss_parts <= 1) or the sum of the q_ss_parts partials
  * q_sumsq[r * q_ss_ld + 0 .. q_ss_parts) in index order; i.e. Q holds the UN-normalised projection and q_sumsq the row
- * sums of squares the GEMM epilogue produced (svi_gemm_epilogue.sumsq / sumsq_parts).  The norm's per-channel weight commutes with
- * the dot product and is applied to K by the caller (K' = K * w_q).  Replaces norm_q of CrossAttention.forward,
+ * sums of squares the GEMM epilogue produced (svi_gemm_epilogue.sumsq / sumsq_parts); q_sumsq must be 4-byte aligned.
+ * The norm's per-channel weight commutes with the dot product and is applied to K by the caller (K' = K * w_q).  Replaces norm_q of CrossAttention.forward,
  * wan_video_dit.py:272, without a pass over Q.
  */
 int svi_attn_fwd_qscale(const void* Q, int64_t ldq, const void* K, int64_t ldk, const void* V, int64_t ldv,
@@ -137,7 +143,7 @@ void svi_attn_plan(int32_t units, int32_t kv_tiles, int32_t sms, size_t workspac
  *                [c*kv_chunk_rows, (c+1)*kv_chunk_rows) are produced by rank c: the K/V stream starts on the local
  *                chunk kv_self_chunk and the TMA producer waits for kv_flags[c] == kv_epoch (ld.acquire.sys) before
  *                the first tile that touches chunk c, so the push of the remote rows overlaps the attention math.
- *                kv_flags: device uint32[n_chunks] inside this rank's symmetric allocation.
+ *                kv_flags: device uint32[n_chunks] inside this rank's symmetric allocation, 4-byte aligned.
  * Flags are compared for equality: the caller alternates two buffers/flag arrays by layer parity and numbers the
  * launches 1,2,3,... so a flag cannot advance past the epoch a consumer still waits for (DESIGN.md §6).
  */
@@ -348,7 +354,8 @@ int svi_softmax_rows(const float* s, int32_t rows, int32_t N, int64_t lds, float
  *                       bias_table f32 [n_buckets, H] + bucket int32 [Lq, Lk] (T5RelativeEmbedding :159-190, the
  *                       bucket of (query, key) is position-only and shared by all layers) or both NULL;
  *                       key_mask int32 [Lk] (0 = masked; T5Attention :73-77) or NULL; with every key masked the
- *                       output rows are 0 (not the NaN of a softmax over an empty set).
+ *                       output rows are 0 (not the NaN of a softmax over an empty set).  bias_table, bucket and
+ *                       key_mask must be 4-byte aligned.
  *                       Replaces T5Attention.forward :55-89 (scale 1, bias, mask) and the CLIP SelfAttention
  *                       (wan_video_image_encoder.py:255-268: head_dim 80, scale 1/sqrt(80)).
  */

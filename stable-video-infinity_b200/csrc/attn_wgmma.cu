@@ -381,6 +381,10 @@ static int launch_attn(const void* Q, int64_t ldq, const void* K, int64_t ldk, c
   SVI_REQUIRE(((reinterpret_cast<uintptr_t>(Q) | reinterpret_cast<uintptr_t>(K) |
                 reinterpret_cast<uintptr_t>(V) | reinterpret_cast<uintptr_t>(O)) & 15) == 0,
               "%s: pointers must be 16-byte aligned", who);
+  SVI_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15) == 0, "%s: workspace must be 16-byte aligned", who);
+  // read with 4-byte scalar loads (ld.acquire.sys.u32 / __ldg)
+  SVI_REQUIRE((reinterpret_cast<uintptr_t>(kv_flags) & 3) == 0, "%s: kv_flags must be 4-byte aligned", who);
+  SVI_REQUIRE((reinterpret_cast<uintptr_t>(qs.sumsq) & 3) == 0, "%s: q_sumsq must be 4-byte aligned", who);
   CUtensorMap tq, tk, tv;
   int rc = make_tmap_2d(&tq, Q, 2, (uint64_t)width, (uint64_t)Lq, (uint64_t)ldq * 2, 64, BQ);
   if (rc) return rc;
@@ -425,7 +429,6 @@ static int launch_attn(const void* Q, int64_t ldq, const void* K, int64_t ldk, c
   const int units = p.n_qtiles * num_heads;
   const int sms = sm_count();
   if (sms <= 0) return SVI_ERR_DRIVER;
-  SVI_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15) == 0, "%s: workspace must be 16-byte aligned", who);
   plan_split(units, (Lk + BKV - 1) / BKV, sms, (workspace && !accumulate) ? workspace_bytes : 0, &p.n_full, &p.split);
   const int n_sliced = units - p.n_full;
   const long long slices = (long long)n_sliced * p.split;

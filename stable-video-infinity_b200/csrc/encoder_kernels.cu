@@ -258,6 +258,10 @@ extern "C" int svi_attn_small(const void* Q, int64_t ldq, const void* K, int64_t
   SVI_REQUIRE((bias_table == nullptr) == (bucket == nullptr), "svi_attn_small: bias_table and bucket go together");
   const int64_t width = (int64_t)num_heads * head_dim;
   SVI_REQUIRE(ldq >= width && ldk >= width && ldv >= width && ldo >= width, "svi_attn_small: leading dimensions too small");
+  // read with 4-byte scalar loads
+  SVI_REQUIRE((reinterpret_cast<uintptr_t>(bias_table) & 3) == 0, "svi_attn_small: bias_table must be 4-byte aligned");
+  SVI_REQUIRE((reinterpret_cast<uintptr_t>(bucket) & 3) == 0, "svi_attn_small: bucket must be 4-byte aligned");
+  SVI_REQUIRE((reinterpret_cast<uintptr_t>(key_mask) & 3) == 0, "svi_attn_small: key_mask must be 4-byte aligned");
   enc::SmallAttnParams p;
   p.Q = reinterpret_cast<const __nv_bfloat16*>(Q);
   p.K = reinterpret_cast<const __nv_bfloat16*>(K);

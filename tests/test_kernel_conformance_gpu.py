@@ -8,8 +8,8 @@ it is larger than the width.  Three bars, by kind of kernel:
     fp32 ulps of the row's scale (cancellation near zero).  The fp32 results differ by reassociation and by the MUFU
     exp / rcp / rsqrt approximations (~1e-6 relative, common.cuh), below a bf16 ulp, so at most one rounding can flip;
   - fp32 outputs: a few fp32 ulps of the magnitude of the terms (FMA contraction, reassociation).
-GEMM and attention keep tolerance bars here; their sharp checks are the gemm_edges / attn_online / attn_small_long
-sections of tools/gpu_check.py.  Every bar has a negative control: a wrong but plausible reference must fail it.
+GEMM and attention keep tolerance bars here; their sharp checks are the gemm_edges section of tools/gpu_check.py and the
+per-element fp64 bars of tests/test_attention_fp64_gpu.py.  Every bar has a negative control: a wrong but plausible reference must fail it.
 
 COVERED / EXEMPT list every entry point of include/svi_b200.h; tests/test_kernel_coverage_cpu.py fails when one is missing.
 This module imports without a GPU.
@@ -24,13 +24,16 @@ import nv_emulation as E
 import nv_emulation_audio as EA
 from diffsynth import _native as nv
 
-# entry point -> the cases that run it: "A:<test function of this module>" or "B:<tools/gpu_check.py section>"
+# entry point -> the cases that run it: "A:<test function of this module>", "B:<tools/gpu_check.py section>" or
+# "F:<test function of tests/test_attention_fp64_gpu.py>"
 COVERED = {
     "svi_gemm_bf16": ("A:test_gemm_matches_standin", "B:gemm", "B:gemm_epi", "B:gemm_edges", "B:ln_fold"),
-    "svi_attn_fwd": ("A:test_attention_matches_standin", "B:attn", "B:attn_online", "B:attn_bench"),
-    "svi_attn_workspace_bytes": ("B:attn", "B:attn_online", "B:attn_sp_one_gpu"),
-    "svi_attn_fwd_qscale": ("A:test_attention_matches_standin", "B:abi3"),
-    "svi_attn_fwd_sp": ("B:attn_sp_one_gpu",),
+    "svi_attn_fwd": ("A:test_attention_matches_standin", "B:attn", "B:attn_online", "B:attn_bench", "F:test_attention_case",
+                     "F:test_accumulate_image_branch", "F:test_bench_shape_sampled", "F:test_engine_launches"),
+    "svi_attn_workspace_bytes": ("B:attn", "B:attn_online", "B:attn_sp_one_gpu", "F:test_attention_case", "F:test_sp_one_gpu"),
+    "svi_attn_fwd_qscale": ("A:test_attention_matches_standin", "B:abi3", "F:test_qscale_layouts", "F:test_engine_launches"),
+    "svi_attn_fwd_sp": ("B:attn_sp_one_gpu", "F:test_sp_one_gpu"),
+    "svi_attn_plan": ("F:test_plans_are_distinct", "F:test_attention_case"),
     "svi_layernorm_modulate": ("A:test_layernorm_modulate",),
     "svi_layernorm_modulate_split": ("A:test_split_forms",),
     "svi_rmsnorm_rope": ("A:test_rmsnorm_rope",),
@@ -61,7 +64,7 @@ COVERED = {
     "svi_rmsnorm_affine": ("A:test_encoder_norms",),
     "svi_layernorm_f32": ("A:test_encoder_norms",),
     "svi_mul_bf16": ("A:test_small_data_movement",),
-    "svi_attn_small": ("A:test_attention_small_matches_standin", "B:attn_small_long"),
+    "svi_attn_small": ("A:test_attention_small_matches_standin", "B:attn_small_long", "F:test_attention_small_case"),
     "svi_col_stats_workspace_bytes": ("A:test_col_stats",),
     "svi_col_stats": ("A:test_col_stats",),
     "svi_col_norm_act": ("A:test_col_norm_act",),
@@ -72,7 +75,6 @@ EXEMPT = {
     "svi_abi_version": "constant; checked by build()",
     "svi_last_error": "message accessor; every wrapper reads it when a call fails",
     "svi_sm_count": "device query; every grid-capped launch uses it",
-    "svi_attn_plan": "host-only launch plan; test_properties_cpu.py::test_attention_plan_invariants",
     "svi_sp_alloc": "needs two GPUs (test_sp_gpu.py)",
     "svi_sp_free": "needs two GPUs (test_sp_gpu.py)",
     "svi_sp_open": "needs two GPUs (test_sp_gpu.py)",

@@ -5,6 +5,7 @@ case fails here, on the CPU, before anyone runs the GPU suite."""
 import os
 import re
 
+import test_attention_fp64_gpu as attn64
 import test_kernel_conformance_gpu as conf
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -46,17 +47,18 @@ def test_every_entry_point_has_a_case_or_an_exemption():
 
 def test_named_cases_exist():
     """A:<name> is a test function of the conformance module; B:<name> is a tools/gpu_check.py section that
-    tests/test_kernels_gpu.py runs."""
+    tests/test_kernels_gpu.py runs; F:<name> is a test function of tests/test_attention_fp64_gpu.py."""
     gpu_check = _read("tools", "gpu_check.py")
     sections = _read("tests", "test_kernels_gpu.py")
     for entry, cases in conf.COVERED.items():
         assert cases, f"{entry}: empty case list"
         for case in cases:
             kind, name = case.split(":", 1)
-            if kind == "A":
-                assert callable(getattr(conf, name, None)) and name.startswith("test_"), f"{entry}: no test {name}"
+            if kind in ("A", "F"):
+                mod = conf if kind == "A" else attn64
+                assert callable(getattr(mod, name, None)) and name.startswith("test_"), f"{entry}: no test {name}"
             else:
-                assert kind == "B", f"{entry}: case {case} is neither A: nor B:"
+                assert kind == "B", f"{entry}: case {case} is neither A:, B: nor F:"
                 assert re.search(rf"^def sec_{name}\(", gpu_check, re.M), f"{entry}: gpu_check has no section {name}"
                 assert f'"{name}"' in sections, f"{entry}: test_kernels_gpu.py does not run section {name}"
 

@@ -587,6 +587,19 @@ def sec_gemm_edges():
     _gemm_bound_report("gemm_edges bf16 M=2048 N=4608 K=136 (every CTA loops)", out, a3, w3, 136)
 
 
+def attn_online_inputs(g, Lq, Lk, H, amp, ramp=0.0, dominant=None):
+    """bf16 q, k, v of the online-softmax stresses: every score gains ramp * key / (Lk - 1) (with scale 1/sqrt(128), so the
+    row max rises in every K/V tile), and key `dominant`, when given, gains +35 on every score"""
+    q = torch.randn(Lq, H * 128, generator=g) * amp
+    k = torch.randn(Lk, H * 128, generator=g) * amp
+    v = torch.randn(Lk, H * 128, generator=g)
+    q.view(Lq, H, 128)[:, :, 0] = 4.0                   # a common direction: scores rise with k[:, 0]
+    k.view(Lk, H, 128)[:, :, 0] += ramp * torch.arange(Lk).float().unsqueeze(1) / max(Lk - 1, 1)
+    if dominant is not None:
+        k.view(Lk, H, 128)[dominant, :, 0] = 100.0     # +35 on every score of that key
+    return tuple(t.to(dev, torch.bfloat16) for t in (q, k, v))
+
+
 def sec_attn_online():
     """Online softmax under stress (bar: report()'s elementwise min_inside against the fp32 reference): key amplitude
     growing along the sequence so the row max rises in every K/V tile, one dominant key in the last tile or in a middle slice
@@ -596,14 +609,7 @@ def sec_attn_online():
     scale = 128 ** -0.5
 
     def make(Lq, Lk, H, amp, ramp=0.0, dominant=None):
-        q = torch.randn(Lq, H * 128, generator=g) * amp
-        k = torch.randn(Lk, H * 128, generator=g) * amp
-        v = torch.randn(Lk, H * 128, generator=g)
-        q.view(Lq, H, 128)[:, :, 0] = 4.0                   # a common direction: scores rise with k[:, 0]
-        k.view(Lk, H, 128)[:, :, 0] += ramp * torch.arange(Lk).float().unsqueeze(1) / max(Lk - 1, 1)
-        if dominant is not None:
-            k.view(Lk, H, 128)[dominant, :, 0] = 100.0     # +35 on every score of that key
-        return (t.to(dev, torch.bfloat16) for t in (q, k, v))
+        return attn_online_inputs(g, Lq, Lk, H, amp, ramp, dominant)
 
     cases = [("ramp", 1000, 1000, 2, 3.5, 120.0, None), ("ramp sliced", 3200, 4100, 12, 3.5, 120.0, None),
              ("dominant key in the last tile", 700, 1000, 2, 3.2, 0.0, 999),
