@@ -1,17 +1,22 @@
 // Persistent warp-specialised bf16 GEMM for sm_90a:  out = epilogue(A[M,K] @ W[N,K]^T).
 //
-//   warpgroup 0     : TMA producer (one lane; 128B-swizzled 128x64 A and 256x64 W tiles into a 4-stage ring), 40 registers
-//   warpgroups 1, 2 : consumers, rows [0, 64) and [64, 128) of the 128 x 256 tile: wgmma m64n256k16 with the fp32
-//                     accumulator in registers, then the epilogue straight from those registers, 232 registers
+//   warpgroup 0     : TMA producer (one lane; 128B-swizzled 128x64 A and 128x64 W tiles into a 6-stage ring), 40 registers
+//   warpgroups 1, 2 : consumers in ping-pong: each owns whole 128 x 128 tiles (the CTA's even and odd tiles), as two
+//                     m64n128k16 row halves with the fp32 accumulator in registers, then runs the epilogue straight from
+//                     those registers, 232 registers
+//
+// The ring is filled in tile order and each tile's k-blocks belong to one warpgroup; an ordering barrier hands the ring
+// from one warpgroup to the other after each mainloop, so the mainloops alternate: while one warpgroup runs its epilogue
+// (bias, activation, residual loads, stores), the other's MMAs keep the tensor cores busy.
 //
 // e4m3 weights (svi_gemm_epilogue.w_e4m3 = 1; the reference's weight-only FP8 mode): the producer lane TMA-loads the
-// 256 x 64 e4m3 W tile (16 KB, unswizzled) into a staging ring instead, and warps 1-3 of warpgroup 0 (idle in the bf16
+// 128 x 64 e4m3 W tile (8 KB, unswizzled) into a staging ring instead, and warps 1-3 of warpgroup 0 (idle in the bf16
 // instantiation) convert it, exactly, into the bf16 W tile in the same 128B-swizzled layout the bf16 TMA load produces.
 // The consumers, their wgmma descriptors and the epilogue are the same code, so the result is bit-identical to the bf16
-// GEMM on bf16(W).  Shared memory: 3 bf16 stages (144 KB) + 4 staging stages (64 KB) = 208 KB, against 4 x 48 KB for bf16.
+// GEMM on bf16(W).  Shared memory: 5 bf16 stages (160 KB) + 4 staging stages (32 KB), against 6 x 32 KB for bf16.
 //
-// The producer runs ahead into the next tile while the consumers drain the previous one, so operand loads overlap the
-// epilogue.  Tiles are visited in groups of GROUP_M row blocks so that the CTAs resident together share A and W tiles in L2.
+// The producer runs ahead across tiles, so operand loads overlap the epilogues.  Tiles are visited in groups of GROUP_M
+// row blocks so that the CTAs resident together share A and W tiles in L2.
 // Replaces every F.linear of the reference's DiT (see include/svi_b200.h for the line map).
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -21,22 +26,24 @@ namespace svi {
 namespace gemm {
 
 constexpr int BM = 128;
-constexpr int BN = 256;
+constexpr int BN = 128;
 constexpr int BK = 64;  // 64 bf16 = 128 B = one swizzle row
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
-constexpr int B_STAGE_BYTES = BN * BK * 2;  // 32 KB
+constexpr int B_STAGE_BYTES = BN * BK * 2;  // 16 KB
 constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-constexpr int W8_STAGE_BYTES = BN * BK;     // 16 KB of e4m3 W
+constexpr int W8_STAGE_BYTES = BN * BK;     // 8 KB of e4m3 W
 constexpr int NUM_THREADS = 384;
 constexpr int NUM_CONVERTERS = 96;          // warps 1-3 of warpgroup 0 (e4m3 instantiation)
 constexpr int GROUP_M = 8;
+constexpr int RES_J = 4;                    // 8-column blocks whose residual, bias and gate loads go out together
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 65536
 static_assert(A_STAGE_BYTES % 1024 == 0 && STAGE_BYTES % 1024 == 0, "operand tiles must stay 1024-byte aligned");
+static_assert((BN / 8) % RES_J == 0, "residual batches must tile the warp's columns");
 
 // Ring depths per weight format: bf16 stages (A + bf16 W) and e4m3 staging stages.
 template <bool kE4M3> struct Rings;
-template <> struct Rings<false> { static constexpr int STAGES = 4, W8_STAGES = 0; };
-template <> struct Rings<true> { static constexpr int STAGES = 3, W8_STAGES = 4; };
+template <> struct Rings<false> { static constexpr int STAGES = 6, W8_STAGES = 0; };
+template <> struct Rings<true> { static constexpr int STAGES = 5, W8_STAGES = 4; };
 template <bool kE4M3>
 constexpr int smem_bytes() {
   return Rings<kE4M3>::STAGES * STAGE_BYTES + Rings<kE4M3>::W8_STAGES * W8_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
@@ -63,7 +70,7 @@ __device__ __forceinline__ uint2 e4m3x4_to_bf16x4(uint32_t w) {
   return make_uint2(lo, hi);
 }
 
-// One 256 x 64 e4m3 staging tile (row-major, 64 B per row) -> the bf16 W tile as the 128B-swizzled TMA load lays it out:
+// One 128 x 64 e4m3 staging tile (row-major, 64 B per row) -> the bf16 W tile as the 128B-swizzled TMA load lays it out:
 // row r at byte 128 r, its 16-byte chunk j at chunk position j ^ (r & 7).  Thread t takes 16-byte source chunks t, t + 96, ...
 // (row i / 4, bf16 chunks 2 (i % 4) and 2 (i % 4) + 1); a quarter-warp's stores hit eight distinct bank groups.
 __device__ __forceinline__ void convert_w_tile(uint32_t src, uint32_t dst, int t) {
@@ -84,8 +91,6 @@ __device__ __forceinline__ void convert_w_tile(uint32_t src, uint32_t dst, int t
 struct Epi {
   void* out;
   long long ldo;
-  int out_is_f32;
-  int act;
   const float* bias;
   const float* gate;
   const float* residual;
@@ -107,6 +112,10 @@ struct Epi {
   float* row_stats;        // [M, 2] += (sum v, sum v^2) over this launch's columns (atomicAdd)
 };
 
+// Named barriers 1 and 2 between the two consumer warpgroups (128 threads wait, the other 128 arrive).
+__device__ __forceinline__ void named_bar_sync(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id) { asm volatile("bar.arrive %0, 256;" ::"r"(id) : "memory"); }
+
 __device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int& m_blk, int& n_blk) {
   const int per_group = GROUP_M * num_n;
   const int g = tile / per_group;
@@ -117,15 +126,19 @@ __device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int&
   n_blk = idx / rows;
 }
 
-// Activation with the switch outside the element loop (act is uniform over the launch).
-__device__ __forceinline__ void apply_act2(float& a, float& b, int act) {
-  if (act == SVI_ACT_GELU_TANH) {
+// The activation, the output type and the LayerNorm fold are template parameters of the kernel: the epilogue is unrolled
+// over all 64 accumulator pairs of a warp's slice, so runtime switches put the code of every variant into that unrolled
+// body.  One kernel held about 17 000 SASS instructions that way, and at K = 1536 the bare GEMM ran at 190 TFLOP/s against
+// 490 with one kernel per variant (H100 80GB HBM3, 700 W, tools/gemm_bench.py).
+template <int kAct>
+__device__ __forceinline__ void apply_act2(float& a, float& b) {
+  if constexpr (kAct == SVI_ACT_GELU_TANH) {
     a = gelu_tanh(a); b = gelu_tanh(b);
-  } else if (act == SVI_ACT_SILU) {
+  } else if constexpr (kAct == SVI_ACT_SILU) {
     a = silu(a); b = silu(b);
-  } else if (act == SVI_ACT_GELU_ERF) {
+  } else if constexpr (kAct == SVI_ACT_GELU_ERF) {
     a = gelu_erf(a); b = gelu_erf(b);
-  } else if (act == SVI_ACT_RELU) {
+  } else if constexpr (kAct == SVI_ACT_RELU) {
     a = fmaxf(a, 0.f); b = fmaxf(b, 0.f);
   }
 }
@@ -152,13 +165,17 @@ __device__ __forceinline__ void sumsq_flush(const Epi& ep, int row, bool ok, int
   }
 }
 
-// Epilogue of one warp's 16 x 256 accumulator slice: rows row0 + g and row0 + g + 8, columns n_base + 8j + 2c (+1).
+// Epilogue of one warp's 16 x 128 accumulator slice: rows row0 + g and row0 + g + 8, columns n_base + 8j + 2c (+1).
+// The residual may be `out` itself (each element is read and then written by the same lane only), so the compiler may not
+// move a load above an earlier store: the residual, bias and gate loads of RES_J column blocks are issued together, ahead
+// of their stores, which makes one memory round trip per batch instead of one per column block.
+template <int kAct, bool kF32, bool kFold>
 __device__ __forceinline__ void epilogue(const Epi& ep, float (&acc)[BN / 2], int M, int N, int row0, int n_base, int lane) {
   const int g = lane >> 2, c = lane & 3;
   const int rows[2] = {row0 + g, row0 + g + 8};
   const bool ok[2] = {rows[0] < M, rows[1] < M};
   float ln_r[2] = {1.f, 1.f}, ln_nmu[2] = {0.f, 0.f};
-  if (ep.ln_stats) {
+  if (kFold && ep.ln_stats) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (!ok[h]) continue;
@@ -171,12 +188,37 @@ __device__ __forceinline__ void epilogue(const Epi& ep, float (&acc)[BN / 2], in
   float ss[2] = {0.f, 0.f};
   int key = -1;
   float ps[2] = {0.f, 0.f}, pq[2] = {0.f, 0.f};
+  float2 res[RES_J][2], bvs[RES_J], gvs[RES_J];
+  // this lane's first column in each of its two rows: column block j is then a constant offset of 8 j elements
+  const long long col0 = (long long)n_base + 2 * c;
+  const float* res_row[2];
+  void* out_row[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    res_row[h] = ep.residual ? ep.residual + rows[h] * ep.ldr + col0 : nullptr;
+    out_row[h] = kF32 ? (void*)(reinterpret_cast<float*>(ep.out) + rows[h] * ep.ldo + col0)
+                      : (void*)(reinterpret_cast<__nv_bfloat16*>(ep.out) + rows[h] * ep.ldo + col0);
+  }
 #pragma unroll
   for (int j = 0; j < BN / 8; ++j) {
+    if (j % RES_J == 0) {
+#pragma unroll
+      for (int i = 0; i < RES_J; ++i) {
+        const int nb = n_base + 8 * (j + i);
+        const bool in = nb < N;
+        bvs[i] = ep.bias && in ? __ldg(reinterpret_cast<const float2*>(ep.bias + nb + 2 * c)) : make_float2(0.f, 0.f);
+        gvs[i] = ep.gate && in ? __ldg(reinterpret_cast<const float2*>(ep.gate + nb + 2 * c)) : make_float2(1.f, 1.f);
+        if (ep.residual) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            res[i][h] = ok[h] && in ? *reinterpret_cast<const float2*>(res_row[h] + 8 * (j + i)) : make_float2(0.f, 0.f);
+        }
+      }
+    }
     const int n0 = n_base + 8 * j;
     if (n0 < N) {   // warp-uniform (N % 8 == 0)
       const int n = n0 + 2 * c;
-      if (ep.sumsq) {
+      if (ep.sumsq && j % 4 == 0) {   // a group starts only on a 32-column boundary (sumsq_group_cols % 32 == 0)
         const int k = ep.sumsq_parts ? (n0 >> 7) : n0 / ep.sumsq_group_cols;
         if (k != key) {
           sumsq_flush(ep, rows[0], ok[0], lane, ss[0], key);
@@ -185,36 +227,33 @@ __device__ __forceinline__ void epilogue(const Epi& ep, float (&acc)[BN / 2], in
           key = k;
         }
       }
-      const float2 bv = ep.bias ? __ldg(reinterpret_cast<const float2*>(ep.bias + n)) : make_float2(0.f, 0.f);
-      const float2 gv = ep.gate ? __ldg(reinterpret_cast<const float2*>(ep.gate + n)) : make_float2(1.f, 1.f);
-      const float2 uv = ep.ln_stats ? __ldg(reinterpret_cast<const float2*>(ep.ln_u + n)) : make_float2(0.f, 0.f);
-      const float2 gn = ep.a_next ? __ldg(reinterpret_cast<const float2*>(ep.g_next + n)) : make_float2(0.f, 0.f);
+      const float2 bv = bvs[j % RES_J], gv = gvs[j % RES_J];
+      const float2 uv = kFold && ep.ln_stats ? __ldg(reinterpret_cast<const float2*>(ep.ln_u + n)) : make_float2(0.f, 0.f);
+      const float2 gn = kFold && ep.a_next ? __ldg(reinterpret_cast<const float2*>(ep.g_next + n)) : make_float2(0.f, 0.f);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-        if (ep.ln_stats) {
+        if (kFold && ep.ln_stats) {
           v0 = ln_r[h] * fmaf(ln_nmu[h], uv.x, v0);
           v1 = ln_r[h] * fmaf(ln_nmu[h], uv.y, v1);
         }
         v0 += bv.x; v1 += bv.y;
-        if (ep.act != SVI_ACT_NONE) apply_act2(v0, v1, ep.act);
+        apply_act2<kAct>(v0, v1);
         ss[h] += fmaf(v0, v0, v1 * v1);   // contraction spelled out: identical in both weight-format instantiations
         v0 *= gv.x; v1 *= gv.y;
         if (ok[h]) {
           if (ep.residual) {
-            const float2 r = *reinterpret_cast<const float2*>(ep.residual + (long long)rows[h] * ep.ldr + n);
-            v0 += r.x; v1 += r.y;
+            v0 += res[j % RES_J][h].x; v1 += res[j % RES_J][h].y;
           }
-          if (ep.a_next) {
+          if (kFold && ep.a_next) {
             ps[h] += v0 + v1;
             pq[h] = fmaf(v1, v1, fmaf(v0, v0, pq[h]));
             *reinterpret_cast<uint32_t*>(ep.a_next + (long long)rows[h] * ep.ld_an + n) = pack_bf16x2(v0 * gn.x, v1 * gn.y);
           }
-          if (ep.out_is_f32) {
-            *reinterpret_cast<float2*>(reinterpret_cast<float*>(ep.out) + (long long)rows[h] * ep.ldo + n) = make_float2(v0, v1);
+          if constexpr (kF32) {
+            *reinterpret_cast<float2*>(reinterpret_cast<float*>(out_row[h]) + 8 * j) = make_float2(v0, v1);
           } else {
-            *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.out) + (long long)rows[h] * ep.ldo + n) =
-                pack_bf16x2(v0, v1);
+            *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(out_row[h]) + 8 * j) = pack_bf16x2(v0, v1);
           }
         }
       }
@@ -224,7 +263,7 @@ __device__ __forceinline__ void epilogue(const Epi& ep, float (&acc)[BN / 2], in
     sumsq_flush(ep, rows[0], ok[0], lane, ss[0], key);
     sumsq_flush(ep, rows[1], ok[1], lane, ss[1], key);
   }
-  if (ep.a_next) {
+  if (kFold && ep.a_next) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const float a = quad_sum(ps[h]), b = quad_sum(pq[h]);
@@ -236,7 +275,7 @@ __device__ __forceinline__ void epilogue(const Epi& ep, float (&acc)[BN / 2], in
   }
 }
 
-template <bool kE4M3>
+template <bool kE4M3, int kAct, bool kF32, bool kFold>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, int M, int N, int K,
                  const __grid_constant__ Epi ep) {
@@ -263,7 +302,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     tma_prefetch_desc(&tmap_b);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init_a(full_bar(i), kE4M3 ? 1 + NUM_CONVERTERS / 32 : 1);   // e4m3: + one arrive per converter warp
-      mbar_init_a(empty_bar(i), 8);   // one arrive per consumer warp
+      mbar_init_a(empty_bar(i), 4);   // one arrive per warp of the consumer warpgroup that owns the stage's tile
     }
     for (int i = 0; i < W8_STAGES; ++i) {
       mbar_init_a(full8_bar(i), 1);
@@ -326,43 +365,62 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   } else {
     // ------------------------------- consumers ----------------------------------
     setmaxnreg_inc<CONSUMER_REGS>();
-    const int cw = wg - 1;   // rows [64 cw, 64 cw + 64) of the tile
+    // Warpgroup cw takes the CTA's tiles 2 i + cw.  The ring holds the tiles' k-blocks in the producer's order, so each
+    // warpgroup steps over the other's num_k stages after every tile of its own (and warpgroup 1 before its first).
+    const int cw = wg - 1;
     int stage = 0;
     uint32_t phase = 0;
-    float acc[BN / 2];
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    auto skip_tile = [&]() {
+      const int s = stage + num_k;
+      phase ^= (uint32_t)(s / STAGES) & 1u;
+      stage = s % STAGES;
+    };
+    if (cw == 1) skip_tile();
+    float acc[2][BN / 2];   // rows [0, 64) and [64, 128) of the tile
+    for (int tile = blockIdx.x + cw * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x) {
       int m_blk, n_blk;
       tile_coords(tile, num_m, num_n, m_blk, n_blk);
+      // Ordering barrier (named barrier 1 + cw): a warpgroup starts waiting on the ring only after the other one has waited
+      // on every k-block before its tile, so no full-barrier wait runs more than one phase ahead (the parity would alias).
+      if (tile != (int)blockIdx.x) named_bar_sync(1 + cw);
       int prev = -1;
       for (int kb = 0; kb < num_k; ++kb) {
         mbar_wait_a(full_bar(stage), phase);
         const uint32_t sa = sbase + stage * STAGE_BYTES;
-        const uint64_t da = wgmma_desc(sa + cw * 64 * 128, 16, 1024);
+        const uint64_t da0 = wgmma_desc(sa, 16, 1024);
+        const uint64_t da1 = wgmma_desc(sa + 64 * 128, 16, 1024);
         const uint64_t db = wgmma_desc(sa + A_STAGE_BYTES, 16, 1024);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k)   // +32 B per K-step = +2 in the 16-byte address field
-          Wgmma<BN>::ss(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
+        for (int k = 0; k < BK / 16; ++k) {   // +32 B per K-step = +2 in the 16-byte address field
+          Wgmma<BN>::ss(acc[0], da0 + 2 * k, db + 2 * k, (kb | k) != 0);
+          Wgmma<BN>::ss(acc[1], da1 + 2 * k, db + 2 * k, (kb | k) != 0);
+        }
         wgmma_commit();
         wgmma_wait<1>();   // the previous stage's MMAs have retired: its slot goes back to the producer
         if (prev >= 0 && lane == 0) mbar_arrive_a(empty_bar(prev));
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      if (tile + (int)gridDim.x < num_tiles) named_bar_arrive(2 - cw);   // the CTA's next tile is the other warpgroup's
       wgmma_wait<0>();
-      wgmma_fence_regs(acc);
+      wgmma_fence_regs(acc[0]);
+      wgmma_fence_regs(acc[1]);
       if (lane == 0) mbar_arrive_a(empty_bar(prev));
-      epilogue(ep, acc, M, N, m_blk * BM + cw * 64 + (warp & 3) * 16, n_blk * BN, lane);
+      skip_tile();
+      const int row0 = m_blk * BM + (warp & 3) * 16;
+      epilogue<kAct, kF32, kFold>(ep, acc[0], M, N, row0, n_blk * BN, lane);
+      epilogue<kAct, kF32, kFold>(ep, acc[1], M, N, row0 + 64, n_blk * BN, lane);
     }
   }
 }
 
 // Sets the dynamic shared-memory size of one instantiation once per process, then launches it.
-template <bool kE4M3>
+template <bool kE4M3, int kAct, bool kF32, bool kFold>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, const Epi& ep, cudaStream_t stream) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t ce = cudaFuncSetAttribute(gemm_bf16_kernel<kE4M3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t ce = cudaFuncSetAttribute(gemm_bf16_kernel<kE4M3, kAct, kF32, kFold>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           smem_bytes<kE4M3>());
     if (ce != cudaSuccess) {
       set_last_error("svi_gemm_bf16: cudaFuncSetAttribute failed: %s", cudaGetErrorString(ce));
@@ -374,9 +432,31 @@ int launch(const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, co
   const int sms = sm_count();
   if (sms <= 0) return SVI_ERR_DRIVER;
   const int grid = num_tiles < sms ? num_tiles : sms;
-  gemm_bf16_kernel<kE4M3><<<grid, NUM_THREADS, smem_bytes<kE4M3>(), stream>>>(ta, tb, M, N, K, ep);
+  gemm_bf16_kernel<kE4M3, kAct, kF32, kFold><<<grid, NUM_THREADS, smem_bytes<kE4M3>(), stream>>>(ta, tb, M, N, K, ep);
   SVI_CUDA_LAUNCH_CHECK("svi_gemm_bf16");
   return SVI_OK;
+}
+
+template <bool kE4M3, bool kF32, bool kFold>
+int launch_act(const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, int act, const Epi& ep, cudaStream_t stream) {
+  switch (act) {
+    case SVI_ACT_GELU_TANH: return launch<kE4M3, SVI_ACT_GELU_TANH, kF32, kFold>(ta, tb, M, N, K, ep, stream);
+    case SVI_ACT_SILU: return launch<kE4M3, SVI_ACT_SILU, kF32, kFold>(ta, tb, M, N, K, ep, stream);
+    case SVI_ACT_GELU_ERF: return launch<kE4M3, SVI_ACT_GELU_ERF, kF32, kFold>(ta, tb, M, N, K, ep, stream);
+    case SVI_ACT_RELU: return launch<kE4M3, SVI_ACT_RELU, kF32, kFold>(ta, tb, M, N, K, ep, stream);
+    default: return launch<kE4M3, SVI_ACT_NONE, kF32, kFold>(ta, tb, M, N, K, ep, stream);   // act was checked to be in [0, 4]
+  }
+}
+
+// One kernel per (weight format, activation, output type, LayerNorm fold on / off).
+template <bool kE4M3>
+int launch_kind(const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, int act, bool f32, bool fold, const Epi& ep,
+                cudaStream_t stream) {
+  if (f32)
+    return fold ? launch_act<kE4M3, true, true>(ta, tb, M, N, K, act, ep, stream)
+                : launch_act<kE4M3, true, false>(ta, tb, M, N, K, act, ep, stream);
+  return fold ? launch_act<kE4M3, false, true>(ta, tb, M, N, K, act, ep, stream)
+              : launch_act<kE4M3, false, false>(ta, tb, M, N, K, act, ep, stream);
 }
 
 }  // namespace gemm
@@ -432,12 +512,14 @@ extern "C" int svi_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t 
   if (rc) return rc;
 
   Epi ep;
-  ep.out = e->out; ep.ldo = e->ldo; ep.out_is_f32 = e->out_is_f32; ep.act = e->act;
+  ep.out = e->out; ep.ldo = e->ldo;
   ep.bias = e->bias; ep.gate = e->gate; ep.residual = e->residual; ep.ldr = e->ldr;
   ep.sumsq = e->sumsq; ep.sumsq_groups = e->sumsq_groups; ep.sumsq_group_cols = e->sumsq_group_cols; ep.sumsq_parts = e->sumsq_parts;
   ep.ln_stats = e->ln_stats; ep.ln_u = e->ln_u; ep.ln_inv_d = e->ln_dim > 0 ? 1.0f / (float)e->ln_dim : 0.f; ep.ln_eps = e->ln_eps;
   ep.a_next = reinterpret_cast<__nv_bfloat16*>(e->a_next); ep.ld_an = e->ld_an; ep.g_next = e->g_next; ep.row_stats = e->row_stats;
 
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  return e->w_e4m3 ? launch<true>(ta, tb, M, N, K, ep, st) : launch<false>(ta, tb, M, N, K, ep, st);
+  const bool f32 = e->out_is_f32 != 0, fold = e->ln_stats || e->a_next;
+  return e->w_e4m3 ? launch_kind<true>(ta, tb, M, N, K, e->act, f32, fold, ep, st)
+                   : launch_kind<false>(ta, tb, M, N, K, e->act, f32, fold, ep, st);
 }

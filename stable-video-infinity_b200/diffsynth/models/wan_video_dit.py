@@ -259,6 +259,16 @@ class AudioState:
         self.kv = []          # per layer bf16 [n_frames * tokens, 2d]
 
 
+def _gemm_epilogue_class(a, k):
+    """What a gemm call's epilogue does, for the --breakdown tag: o, cross q and cross o share one shape."""
+    out = k.get("out", a[2] if len(a) > 2 else None)
+    parts = [name for name in ("gate", "residual", "sumsq", "ln", "emit") if k.get(name) is not None]
+    if k.get("act", nv.ACT_NONE) != nv.ACT_NONE:
+        parts.append("act")
+    parts.append("f32" if out is not None and out.dtype == torch.float32 else "bf16")
+    return "+".join(parts)
+
+
 class _CountingNative:
     """Proxy over diffsynth._native that counts kernel launches (bench.py reports them as gpu_launches)."""
 
@@ -279,7 +289,7 @@ class _CountingNative:
             e1.record()
             tag = name
             if name == "gemm":
-                tag = f"gemm M={a[0].shape[0]} N={a[1].shape[0]} K={a[1].shape[1]}"
+                tag = f"gemm M={a[0].shape[0]} N={a[1].shape[0]} K={a[1].shape[1]} {_gemm_epilogue_class(a, k)}"
             elif name == "attention":
                 tag = f"attention Lq={a[0].shape[0]} Lk={a[1].shape[0]}"
             self.events.append((tag, e0, e1))
