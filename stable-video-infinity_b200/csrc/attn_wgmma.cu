@@ -2,11 +2,36 @@
 //
 // One CTA owns one 128-row Q tile of one head and streams K/V tiles of 128 rows past it:
 //
-//   warpgroup 0     : TMA producer (one lane: Q once, then K_j / V_j into 2-stage rings, 128B-swizzled boxes)   40 registers
+//   warpgroup 0     : TMA producer (one lane: Q once, then K_j / V_j into 2-stage rings, 128B-swizzled boxes)   24 registers
 //   warpgroups 1, 2 : consumers, 64 Q rows each:  S = Q K_j^T (wgmma, both operands in shared memory, S in registers),
-//                     online softmax in registers, O += P V_j (wgmma with P as the register A operand, V MN-major)  232 registers
+//                     online softmax in registers, O += P V_j (wgmma with P as the register A operand, V MN-major)  240 registers
 //
-// The two consumer warpgroups run independently, so the softmax of one overlaps the tensor-core work of the other.
+// Each consumer pipelines its tiles (`consumer`): after the prologue (S_0 and its softmax), iteration j issues
+// S_j = Q K_j^T and O += P_{j-1} V_{j-1} back to back, waits for S_j only (wgmma_wait<1>), starts the softmax of S_j
+// while P_{j-1} V_{j-1} may still run, then waits for it, rescales O and packs P_j (the registers of P_{j-1} are the A
+// operand of that MMA, so they are overwritten only after it).  O and l evolve as before, in the same order: the output
+// is bit-identical to issuing the two MMAs of a tile one after the other.
+//
+// Ping-pong: the issue of those MMAs alternates between the two consumers through named barriers (warpgroup w waits on
+// barrier 1 + w before it issues, then arrives on the other's), so one warpgroup's MMAs run while the other one does its
+// softmax.  With n = n_kv, each consumer issues n + 1 times (S_0; S_j with P_{j-1} V_{j-1} for j = 1..n-1; P_{n-1} V_{n-1}):
+// warpgroup 1 does not wait before its first issue and warpgroup 2 does not arrive after its last, so each barrier sees
+// as many arrives as waits (n on barrier 1, n + 1 on barrier 2), and the issues go 1, 2, 1, 2, ...  Why this cannot wait
+// in a cycle:
+//   - the producer loads in order K_0, V_0, K_1, V_1, ... and needs K_EMPTY(j-2) before K_j and V_EMPTY(j-2) before V_j,
+//     each from all 8 consumer warps (a slot is released once the MMA reading it has retired);
+//   - a consumer waits for K_j and V_{j-1} BEFORE its barrier wait, and holds the turn only while issuing;
+//   - when a consumer waits for K_j, the other one has issued at least up to S_{j-2} (warpgroup 2 of tile j waits behind
+//     warpgroup 1's issue j; warpgroup 1 behind warpgroup 2's issue j-1), and releases K_{j-2} after its own
+//     wgmma_wait<1> and V_{j-3} after its own wgmma_wait<0>, neither of which waits on anything but its own MMAs; the
+//     waiting consumer released K_{j-1} and V_{j-2} itself.  So every load K_j, V_{j-1} needs will be issued;
+//   - the two consumers are never more than one issue apart, so no mbarrier wait runs a whole phase ahead: each consumer
+//     waits on a slot's full barrier in tile order, and a slot cannot be refilled before all 8 warps released it.
+// Nothing inside this pipeline calls a function or traps (see mbar_wait_pipe), so ptxas keeps the wgmmas asynchronous
+// (WARPGROUP.DEPBAR.LE gsb0, 0x1 after the issue) without spills.  It does move the wait for P_{j-1} V_{j-1} up into
+// the softmax, ahead of its first write to a register of that tile's pipeline (the masked S, or the row maxima / exp2):
+// the overlap inside one warpgroup is partial, and the ping-pong between the two carries most of the gain.
+//
 // Work units are (head, Q tile).  The launch plan (plan_split, host side) runs `n_full` units whole and cuts each of the
 // remaining ones into `split` slices of the K/V stream, so the last, partly filled wave of CTAs is spread over all SMs;
 // sliced units leave (unnormalised O, row max, row sum) in a workspace and attn_merge_kernel combines them.  Without a
@@ -26,7 +51,11 @@ constexpr int KV_STAGES = 2;
 constexpr int HALF_BYTES = 128 * 64 * 2;   // one 128-row x 64-col swizzled box (16 KB)
 constexpr int TILE_BYTES = 2 * HALF_BYTES;  // 128 x 128 bf16 (32 KB)
 constexpr int NUM_THREADS = 384;
-constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+constexpr int PRODUCER_REGS = 24, CONSUMER_REGS = 240;
+// setmaxnreg moves registers inside the CTA's allocation: launch_bounds(384, 1) gives 168 per thread (65536 / 384, in
+// steps of 8), and the consumers can only take what the producer warpgroup gives back
+static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= NUM_THREADS * (65536 / NUM_THREADS / 8 * 8),
+              "register split exceeds the CTA's allocation");
 constexpr uint32_t OFF_Q = 0;
 constexpr uint32_t OFF_K = TILE_BYTES;                          // [KV_STAGES][TILE_BYTES]
 constexpr uint32_t OFF_V = OFF_K + KV_STAGES * TILE_BYTES;      // [KV_STAGES][TILE_BYTES]
@@ -92,6 +121,23 @@ __device__ __forceinline__ void wait_kv_chunk(const uint32_t* flags, int chunk, 
     if (++spins > (1u << 25)) __trap();
   }
   asm volatile("fence.proxy.async.global;" ::: "memory");   // later TMA (async proxy) reads see the pushed rows
+}
+
+// mbar_wait_a without its watchdog, for the consumers' K / V waits: a trap between the wgmma issues and their waits makes
+// ptxas spill the P fragments (208 bytes) and serialise the wgmmas.  A consumer that waits here forever leaves the producer
+// waiting on the same ring's empty barriers, where its own watchdog traps.
+__device__ __forceinline__ void mbar_wait_pipe(uint32_t bar, uint32_t parity) {
+  uint32_t ok = 0;
+  while (!ok)
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
+        "selp.u32 %0, 1, 0, p;\n"
+        "}\n"
+        : "=r"(ok)
+        : "r"(bar), "r"(parity)
+        : "memory");
 }
 
 struct Unit {
@@ -170,32 +216,42 @@ __device__ __forceinline__ void consumer(const Params& p, uint32_t sbase, int cw
 #pragma unroll
   for (int i = 0; i < 64; ++i) o[i] = 0.f;
   const uint32_t q_rows = sbase + OFF_Q + cw * 64 * 128;   // this warpgroup's 64 rows inside each 128-row box
+  float sc[64];        // S_j, then P_j in fp32
+  uint32_t pa[8][4];   // P_{j-1} as bf16 A fragments of the P V MMA
+  const int n = u.n_kv;
+  const int my_bar = 1 + cw, other_bar = 2 - cw;   // named barriers: "warpgroup cw may issue"
 
-  mbar_wait_a(bars + 8 * Q_FULL, 0);
-  for (int j = 0; j < u.n_kv; ++j) {
-    const int s = j % KV_STAGES;
-    const uint32_t ph = (j / KV_STAGES) & 1;
-    float sc[64];
-    mbar_wait_a(bars + 8 * (K_FULL + s), ph);
+  auto wait_full = [&](uint32_t bar, int j) { mbar_wait_pipe(bars + 8 * (bar + j % KV_STAGES), (j / KV_STAGES) & 1); };
+  auto release = [&](uint32_t bar, int j) {
+    if (lane == 0) mbar_arrive_a(bars + 8 * (bar + j % KV_STAGES));
+  };
+  auto issue_qk = [&](int j) {
+    const uint32_t k_tile = sbase + OFF_K + (j % KV_STAGES) * TILE_BYTES;
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < HD / 16; ++kk) {   // 8 K-steps: 4 per 64-column box, +32 B each
       const uint32_t box = (kk >> 2) * HALF_BYTES, koff = (kk & 3) * 32;
-      Wgmma<128>::ss(sc, wgmma_desc(q_rows + box + koff, 16, 1024),
-                     wgmma_desc(sbase + OFF_K + s * TILE_BYTES + box + koff, 16, 1024), kk != 0);
+      Wgmma<128>::ss(sc, wgmma_desc(q_rows + box + koff, 16, 1024), wgmma_desc(k_tile + box + koff, 16, 1024), kk != 0);
     }
     wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(sc);
-    if (lane == 0) mbar_arrive_a(bars + 8 * (K_EMPTY + s));
-
+  };
+  auto issue_pv = [&](int j) {
+    const uint32_t v_tile = sbase + OFF_V + (j % KV_STAGES) * TILE_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int t = 0; t < BKV / 16; ++t)   // 16 K/V rows per step = two 8-row swizzle groups = 2048 B; LBO = next 64 columns
+      Wgmma<128>::rs_tb(o, pa[t], wgmma_desc(v_tile + t * 2048, HALF_BYTES, 1024), 1);
+    wgmma_commit();
+  };
+  // Online softmax of S_j in place: sc = P_j = exp2(S * c - m_new) (masked columns: exp2(-inf) = 0), l = l * alpha + row
+  // sum of P_j; returns alpha = exp2(m_old - m_new) per row half (0 on the first tile, m_old = -inf).
+  auto softmax = [&](int j, float (&alpha)[2]) {
     const int limit = p.Lk - kv_tile_at(u.j_begin + j, p.kv_first_tile, u.n_kv_total) * BKV;  // valid key columns
     if (limit < BKV) {
 #pragma unroll
       for (int i = 0; i < 64; ++i)
         if (8 * (i >> 2) + 2 * c + (i & 1) >= limit) sc[i] = -INFINITY;
     }
-    float alpha[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       float mx = -INFINITY;
@@ -204,32 +260,71 @@ __device__ __forceinline__ void consumer(const Params& p, uint32_t sbase, int cw
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
       const float m_new = fmaxf(m_cur[h], mx * cs[h]);
-      alpha[h] = ex2(m_cur[h] - m_new);   // 0 on the first tile (m_cur = -inf)
+      alpha[h] = ex2(m_cur[h] - m_new);
       m_cur[h] = m_new;
       l[h] *= alpha[h];
     }
-#pragma unroll
-    for (int i = 0; i < 64; ++i) o[i] *= alpha[(i >> 1) & 1];
-    // P = exp2(S * c - m) (masked columns: exp2(-inf) = 0) -> bf16 A fragments of the P V MMA
-    uint32_t pa[8][4];
 #pragma unroll
     for (int i = 0; i < 64; i += 2) {
       const int h = (i >> 1) & 1;
       const float p0 = ex2(fmaf(sc[i], cs[h], -m_cur[h]));
       const float p1 = ex2(fmaf(sc[i + 1], cs[h], -m_cur[h]));
       l[h] += p0 + p1;
-      pa[i >> 3][(i >> 1) & 3] = pack_bf16x2(p0, p1);
+      sc[i] = p0;
+      sc[i + 1] = p1;
     }
-    mbar_wait_a(bars + 8 * (V_FULL + s), ph);
-    wgmma_fence();
+  };
+  auto pack_p = [&]() {
 #pragma unroll
-    for (int t = 0; t < BKV / 16; ++t)   // 16 K/V rows per step = two 8-row swizzle groups = 2048 B; LBO = next 64 columns
-      Wgmma<128>::rs_tb(o, pa[t], wgmma_desc(sbase + OFF_V + s * TILE_BYTES + t * 2048, HALF_BYTES, 1024), 1);
-    wgmma_commit();
+    for (int i = 0; i < 64; i += 2) pa[i >> 3][(i >> 1) & 3] = pack_bf16x2(sc[i], sc[i + 1]);
+  };
+
+  // prologue: S_0 and its softmax (O is still 0: no rescale)
+  mbar_wait_a(bars + 8 * Q_FULL, 0);
+  wait_full(K_FULL, 0);
+  if (cw == 1) named_bar_sync(my_bar);
+  issue_qk(0);
+  named_bar_arrive(other_bar);
+  wgmma_wait<0>();
+  wgmma_fence_regs(sc);
+  release(K_EMPTY, 0);
+  {
+    float alpha[2];
+    softmax(0, alpha);
+  }
+  pack_p();
+  for (int j = 1; j < n; ++j) {
+    wait_full(K_FULL, j);
+    wait_full(V_FULL, j - 1);
+    named_bar_sync(my_bar);
+    issue_qk(j);
+    issue_pv(j - 1);
+    named_bar_arrive(other_bar);
+    wgmma_wait<1>();   // S_j has landed; P_{j-1} V_{j-1} may still run
+    wgmma_fence_regs(sc);
+    release(K_EMPTY, j);
+    float alpha[2];
+    softmax(j, alpha);
+    wgmma_fence_regs(sc);   // the softmax is done before the wait below, not sunk past it
     wgmma_wait<0>();
     wgmma_fence_regs(o);
-    if (lane == 0) mbar_arrive_a(bars + 8 * (V_EMPTY + s));
+    wgmma_fence_regs(sc);   // P_j is packed only after P_{j-1} V_{j-1} has retired
+    release(V_EMPTY, j - 1);
+    // x * 1.0 = x: once the row maxima stop rising the rescale is skipped, warp-uniformly and exactly
+    if (!__all_sync(0xffffffffu, alpha[0] == 1.f && alpha[1] == 1.f)) {
+#pragma unroll
+      for (int i = 0; i < 64; ++i) o[i] *= alpha[(i >> 1) & 1];
+    }
+    pack_p();
   }
+  // epilogue: the last P V
+  wait_full(V_FULL, n - 1);
+  named_bar_sync(my_bar);
+  issue_pv(n - 1);
+  if (cw == 0) named_bar_arrive(other_bar);
+  wgmma_wait<0>();
+  wgmma_fence_regs(o);
+  release(V_EMPTY, n - 1);
 
 #pragma unroll
   for (int h = 0; h < 2; ++h) {

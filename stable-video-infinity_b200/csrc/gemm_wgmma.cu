@@ -112,10 +112,6 @@ struct Epi {
   float* row_stats;        // [M, 2] += (sum v, sum v^2) over this launch's columns (atomicAdd)
 };
 
-// Named barriers 1 and 2 between the two consumer warpgroups (128 threads wait, the other 128 arrive).
-__device__ __forceinline__ void named_bar_sync(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
-__device__ __forceinline__ void named_bar_arrive(int id) { asm volatile("bar.arrive %0, 256;" ::"r"(id) : "memory"); }
-
 __device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int& m_blk, int& n_blk) {
   const int per_group = GROUP_M * num_n;
   const int g = tile / per_group;

@@ -113,6 +113,24 @@ def summarize(rounds):
     return out
 
 
+def alternate(script, lib_args, rounds, args):
+    """Runs `script --one-round ARGS` once per build (--lib NAME=PATH, default the tree's) and round, the builds alternating
+    and the order flipped every round; returns {name: [the JSON each round printed last]}."""
+    libs = [s.split("=", 1) for s in lib_args] or [["tree", ""]]
+    out = {name: [] for name, _ in libs}
+    for r in range(rounds):
+        for name, path in (libs if r % 2 == 0 else libs[::-1]):
+            env = dict(os.environ)
+            if path:
+                env["SVI_B200_LIB"] = os.path.abspath(path)
+            p = subprocess.run([sys.executable, os.path.abspath(script), "--one-round", *args],
+                               env=env, capture_output=True, text=True)
+            if p.returncode != 0:
+                raise SystemExit(f"{os.path.basename(script)}: the {name} round failed:\n{p.stderr[-3000:]}")
+            out[name].append(json.loads(p.stdout.strip().splitlines()[-1]))
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--lib", action="append", default=[], metavar="NAME=PATH",
@@ -124,18 +142,7 @@ def main():
     if a.one_round:
         print(json.dumps(one_round(a.iters)))
         return
-    libs = [s.split("=", 1) for s in a.lib] or [["tree", ""]]
-    rounds = {name: [] for name, _ in libs}
-    for r in range(a.rounds):
-        for name, path in (libs if r % 2 == 0 else libs[::-1]):
-            env = dict(os.environ)
-            if path:
-                env["SVI_B200_LIB"] = os.path.abspath(path)
-            p = subprocess.run([sys.executable, os.path.abspath(__file__), "--one-round", "--iters", str(a.iters)],
-                               env=env, capture_output=True, text=True)
-            if p.returncode != 0:
-                raise SystemExit(f"gemm_bench.py: the {name} round failed:\n{p.stderr[-3000:]}")
-            rounds[name].append(json.loads(p.stdout.strip().splitlines()[-1]))
+    rounds = alternate(__file__, a.lib, a.rounds, ["--iters", str(a.iters)])
     res = {"M": L, "rounds": a.rounds, "builds": {name: summarize(rs) for name, rs in rounds.items()}}
     print(json.dumps(res))
 
