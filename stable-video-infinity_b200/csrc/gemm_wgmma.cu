@@ -18,9 +18,16 @@
 // The producer runs ahead across tiles, so operand loads overlap the epilogues.  Tiles are visited in groups of GROUP_M
 // row blocks so that the CTAs resident together share A and W tiles in L2.
 // Replaces every F.linear of the reference's DiT (see include/svi_b200.h for the line map).
+//
+// LoRA segment (kLoRA, svi_gemm_lora_bf16 in include/svi_b200_lora.h): out = epilogue(A W^T + U_g(n) B^T).  After a tile's
+// num_k k-blocks the producer loads R / 64 more into the same ring, from U [M, groups R] (column g R + 64 kb, g = the
+// tile's column group) and B [N, R]; the consumers run them into the same accumulators, so every epilogue stage sees the
+// LoRA term.  Those tiles are bf16 in both weight formats: with e4m3 W the producer TMA-loads the B tile straight into the
+// swizzled W half and makes the converter warps' arrivals on the stage's full barrier itself; the converters step over it.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "../../include/svi_b200.h"
+#include "../../include/svi_b200_lora.h"
 
 namespace svi {
 namespace gemm {
@@ -111,6 +118,19 @@ struct Epi {
   const float* g_next;     // [N]
   float* row_stats;        // [M, 2] += (sum v, sum v^2) over this launch's columns (atomicAdd)
 };
+
+// The LoRA segment of a launch: empty in the plain instantiations, whose parameter list and code stay as they were.
+template <bool kLoRA> struct LoRAArgs {};
+template <> struct LoRAArgs<true> {
+  CUtensorMap u;    // U [M, groups R] bf16, 64 x 128 boxes, 128B swizzle
+  CUtensorMap b;    // B [N, R] bf16, same boxes
+  int kb;           // R / BK
+  int group_cols;   // 0: one group
+};
+
+__device__ __forceinline__ void mbar_arrive_cnt_a(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
 
 __device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int& m_blk, int& n_blk) {
   const int per_group = GROUP_M * num_n;
@@ -271,10 +291,10 @@ __device__ __forceinline__ void epilogue(const Epi& ep, float (&acc)[BN / 2], in
   }
 }
 
-template <bool kE4M3, int kAct, bool kF32, bool kFold>
+template <bool kE4M3, int kAct, bool kF32, bool kFold, bool kLoRA>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, int M, int N, int K,
-                 const __grid_constant__ Epi ep) {
+                 const __grid_constant__ Epi ep, const __grid_constant__ LoRAArgs<kLoRA> lora) {
   constexpr int STAGES = Rings<kE4M3>::STAGES, W8_STAGES = Rings<kE4M3>::W8_STAGES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -292,6 +312,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const int num_n = (N + BN - 1) / BN;
   const int num_tiles = num_m * num_n;
   const int num_k = (K + BK - 1) / BK;
+  int num_kt = num_k;   // k-blocks per tile, LoRA segment included
+  if constexpr (kLoRA) num_kt += lora.kb;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
@@ -334,6 +356,20 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
+        if constexpr (kLoRA) {
+          const int g = lora.group_cols ? n_blk * BN / lora.group_cols : 0;   // a tile never straddles two groups
+          for (int kb = 0; kb < lora.kb; ++kb) {
+            mbar_wait_a(empty_bar(stage), phase ^ 1);
+            const uint32_t sa = sbase + stage * STAGE_BYTES;
+            // e4m3: no converter touches this stage, so the producer makes their arrivals (before its own, which comes
+            // with the expected bytes: the phase cannot complete before both tiles land)
+            if constexpr (kE4M3) mbar_arrive_cnt_a(full_bar(stage), NUM_CONVERTERS / 32);
+            mbar_expect_tx_a(full_bar(stage), STAGE_BYTES);
+            tma_load_2d_a(sa, &lora.u, full_bar(stage), (g * lora.kb + kb) * BK, m_blk * BM);
+            tma_load_2d_a(sa + A_STAGE_BYTES, &lora.b, full_bar(stage), kb * BK, n_blk * BN);
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          }
+        }
       }
     } else if (kE4M3 && warp >= 1) {
       // ------------------------------- e4m3 -> bf16 W converters -------------------------------
@@ -356,18 +392,19 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           if (++stage8 == W8_STAGES) { stage8 = 0; phase8 ^= 1; }
           if (++stage == STAGES) stage = 0;
         }
+        if constexpr (kLoRA) stage = (stage + lora.kb) % STAGES;   // the LoRA k-blocks arrive in bf16
       }
     }
   } else {
     // ------------------------------- consumers ----------------------------------
     setmaxnreg_inc<CONSUMER_REGS>();
     // Warpgroup cw takes the CTA's tiles 2 i + cw.  The ring holds the tiles' k-blocks in the producer's order, so each
-    // warpgroup steps over the other's num_k stages after every tile of its own (and warpgroup 1 before its first).
+    // warpgroup steps over the other's num_kt stages after every tile of its own (and warpgroup 1 before its first).
     const int cw = wg - 1;
     int stage = 0;
     uint32_t phase = 0;
     auto skip_tile = [&]() {
-      const int s = stage + num_k;
+      const int s = stage + num_kt;
       phase ^= (uint32_t)(s / STAGES) & 1u;
       stage = s % STAGES;
     };
@@ -380,7 +417,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       // on every k-block before its tile, so no full-barrier wait runs more than one phase ahead (the parity would alias).
       if (tile != (int)blockIdx.x) named_bar_sync(1 + cw);
       int prev = -1;
-      for (int kb = 0; kb < num_k; ++kb) {
+      for (int kb = 0; kb < num_kt; ++kb) {
         mbar_wait_a(full_bar(stage), phase);
         const uint32_t sa = sbase + stage * STAGE_BYTES;
         const uint64_t da0 = wgmma_desc(sa, 16, 1024);
@@ -412,12 +449,13 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 }
 
 // Sets the dynamic shared-memory size of one instantiation once per process, then launches it.
-template <bool kE4M3, int kAct, bool kF32, bool kFold>
-int launch(const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, const Epi& ep, cudaStream_t stream) {
+template <bool kE4M3, int kAct, bool kF32, bool kFold, bool kLoRA>
+int launch(const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, const Epi& ep, const LoRAArgs<kLoRA>& lora,
+           cudaStream_t stream) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t ce = cudaFuncSetAttribute(gemm_bf16_kernel<kE4M3, kAct, kF32, kFold>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          smem_bytes<kE4M3>());
+    cudaError_t ce = cudaFuncSetAttribute(gemm_bf16_kernel<kE4M3, kAct, kF32, kFold, kLoRA>,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<kE4M3>());
     if (ce != cudaSuccess) {
       set_last_error("svi_gemm_bf16: cudaFuncSetAttribute failed: %s", cudaGetErrorString(ce));
       return SVI_ERR_LAUNCH;
@@ -428,31 +466,100 @@ int launch(const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, co
   const int sms = sm_count();
   if (sms <= 0) return SVI_ERR_DRIVER;
   const int grid = num_tiles < sms ? num_tiles : sms;
-  gemm_bf16_kernel<kE4M3, kAct, kF32, kFold><<<grid, NUM_THREADS, smem_bytes<kE4M3>(), stream>>>(ta, tb, M, N, K, ep);
+  gemm_bf16_kernel<kE4M3, kAct, kF32, kFold, kLoRA><<<grid, NUM_THREADS, smem_bytes<kE4M3>(), stream>>>(ta, tb, M, N, K, ep, lora);
   SVI_CUDA_LAUNCH_CHECK("svi_gemm_bf16");
   return SVI_OK;
 }
 
-template <bool kE4M3, bool kF32, bool kFold>
-int launch_act(const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, int act, const Epi& ep, cudaStream_t stream) {
-  switch (act) {
-    case SVI_ACT_GELU_TANH: return launch<kE4M3, SVI_ACT_GELU_TANH, kF32, kFold>(ta, tb, M, N, K, ep, stream);
-    case SVI_ACT_SILU: return launch<kE4M3, SVI_ACT_SILU, kF32, kFold>(ta, tb, M, N, K, ep, stream);
-    case SVI_ACT_GELU_ERF: return launch<kE4M3, SVI_ACT_GELU_ERF, kF32, kFold>(ta, tb, M, N, K, ep, stream);
-    case SVI_ACT_RELU: return launch<kE4M3, SVI_ACT_RELU, kF32, kFold>(ta, tb, M, N, K, ep, stream);
-    default: return launch<kE4M3, SVI_ACT_NONE, kF32, kFold>(ta, tb, M, N, K, ep, stream);   // act was checked to be in [0, 4]
+// The LoRA instantiations cover what the DiT blocks use: no activation or GELU-tanh (ffn.0), no LayerNorm fold.
+template <bool kE4M3, bool kF32, bool kFold, bool kLoRA>
+int launch_act(const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, int act, const Epi& ep,
+               const LoRAArgs<kLoRA>& lora, cudaStream_t stream) {
+  if constexpr (kLoRA) {
+    return act == SVI_ACT_GELU_TANH ? launch<kE4M3, SVI_ACT_GELU_TANH, kF32, kFold>(ta, tb, M, N, K, ep, lora, stream)
+                                    : launch<kE4M3, SVI_ACT_NONE, kF32, kFold>(ta, tb, M, N, K, ep, lora, stream);
+  } else {
+    switch (act) {
+      case SVI_ACT_GELU_TANH: return launch<kE4M3, SVI_ACT_GELU_TANH, kF32, kFold>(ta, tb, M, N, K, ep, lora, stream);
+      case SVI_ACT_SILU: return launch<kE4M3, SVI_ACT_SILU, kF32, kFold>(ta, tb, M, N, K, ep, lora, stream);
+      case SVI_ACT_GELU_ERF: return launch<kE4M3, SVI_ACT_GELU_ERF, kF32, kFold>(ta, tb, M, N, K, ep, lora, stream);
+      case SVI_ACT_RELU: return launch<kE4M3, SVI_ACT_RELU, kF32, kFold>(ta, tb, M, N, K, ep, lora, stream);
+      default: return launch<kE4M3, SVI_ACT_NONE, kF32, kFold>(ta, tb, M, N, K, ep, lora, stream);   // act was checked to be in [0, 4]
+    }
   }
 }
 
-// One kernel per (weight format, activation, output type, LayerNorm fold on / off).
-template <bool kE4M3>
+// One kernel per (weight format, activation, output type, LayerNorm fold on / off, LoRA segment on / off).
+template <bool kE4M3, bool kLoRA>
 int launch_kind(const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, int act, bool f32, bool fold, const Epi& ep,
-                cudaStream_t stream) {
-  if (f32)
-    return fold ? launch_act<kE4M3, true, true>(ta, tb, M, N, K, act, ep, stream)
-                : launch_act<kE4M3, true, false>(ta, tb, M, N, K, act, ep, stream);
-  return fold ? launch_act<kE4M3, false, true>(ta, tb, M, N, K, act, ep, stream)
-              : launch_act<kE4M3, false, false>(ta, tb, M, N, K, act, ep, stream);
+                const LoRAArgs<kLoRA>& lora, cudaStream_t stream) {
+  if constexpr (kLoRA) {   // the fold was rejected
+    return f32 ? launch_act<kE4M3, true, false>(ta, tb, M, N, K, act, ep, lora, stream)
+               : launch_act<kE4M3, false, false>(ta, tb, M, N, K, act, ep, lora, stream);
+  } else {
+    if (f32)
+      return fold ? launch_act<kE4M3, true, true>(ta, tb, M, N, K, act, ep, lora, stream)
+                  : launch_act<kE4M3, true, false>(ta, tb, M, N, K, act, ep, lora, stream);
+    return fold ? launch_act<kE4M3, false, true>(ta, tb, M, N, K, act, ep, lora, stream)
+                : launch_act<kE4M3, false, false>(ta, tb, M, N, K, act, ep, lora, stream);
+  }
+}
+
+// The arguments of one GEMM as both entry points take them: checked, then turned into the operand tensor maps and the
+// kernel's epilogue block.  `fn` names the entry point in the messages.
+int prepare(const char* fn, const void* A, int64_t lda, const void* W, int64_t ldw, int32_t M, int32_t N, int32_t K,
+            const svi_gemm_epilogue* e, CUtensorMap* ta, CUtensorMap* tb, Epi* ep) {
+  SVI_REQUIRE(A && W && e && e->out, "%s: null pointer", fn);
+  SVI_REQUIRE(M > 0 && N > 0 && K > 0, "%s: M,N,K must be positive (got %d,%d,%d)", fn, M, N, K);
+  SVI_REQUIRE(K % 8 == 0 && N % 8 == 0, "%s: K and N must be multiples of 8 (K=%d N=%d)", fn, K, N);
+  SVI_REQUIRE(lda % 8 == 0 && ldw % 8 == 0 && lda >= K && ldw >= K, "%s: lda/ldw must be multiples of 8 and >= K", fn);
+  SVI_REQUIRE(e->w_e4m3 == 0 || e->w_e4m3 == 1, "%s: w_e4m3 must be 0 (bf16 W) or 1 (e4m3 W), got %d", fn, e->w_e4m3);
+  if (e->w_e4m3)
+    SVI_REQUIRE(K % 16 == 0 && ldw % 16 == 0,
+                "%s: e4m3 W needs K and ldw to be multiples of 16 (16-byte row pitch; K=%d ldw=%lld)", fn, K, (long long)ldw);
+  SVI_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(W) & 15) == 0,
+              "%s: A and W must be 16-byte aligned", fn);
+  SVI_REQUIRE(e->ldo >= N && e->ldo % (e->out_is_f32 ? 4 : 8) == 0 &&
+                  (reinterpret_cast<uintptr_t>(e->out) & 15) == 0,
+              "%s: out must be 16-byte aligned with ldo >= N and 16-byte row pitch", fn);
+  SVI_REQUIRE(e->act >= 0 && e->act <= 4, "%s: unknown activation %d", fn, e->act);
+  if (e->residual)
+    SVI_REQUIRE(e->ldr >= N && e->ldr % 4 == 0 && (reinterpret_cast<uintptr_t>(e->residual) & 15) == 0,
+                "%s: residual must be 16-byte aligned with ldr >= N, ldr %% 4 == 0", fn);
+  if (e->bias) SVI_REQUIRE((reinterpret_cast<uintptr_t>(e->bias) & 15) == 0, "%s: bias alignment", fn);
+  if (e->gate) SVI_REQUIRE((reinterpret_cast<uintptr_t>(e->gate) & 15) == 0, "%s: gate alignment", fn);
+  if (e->sumsq)
+    SVI_REQUIRE(e->sumsq_groups > 0 && e->sumsq_group_cols > 0 && e->sumsq_group_cols % 32 == 0,
+                "%s: sumsq_group_cols must be a positive multiple of 32", fn);
+  if (e->sumsq && e->sumsq_parts)
+    SVI_REQUIRE(e->sumsq_group_cols % 128 == 0 && e->sumsq_parts == e->sumsq_group_cols / 128,
+                "%s: sumsq_parts must be 0 (atomic accumulation) or sumsq_group_cols / 128 with sumsq_group_cols %% 128 == 0", fn);
+  if (e->ln_stats)
+    SVI_REQUIRE(e->ln_u && e->ln_dim > 0 && (reinterpret_cast<uintptr_t>(e->ln_stats) & 7) == 0 &&
+                    (reinterpret_cast<uintptr_t>(e->ln_u) & 7) == 0,
+                "%s: ln fold needs ln_u (8-byte aligned), ln_dim > 0 and 8-byte aligned ln_stats", fn);
+  if (e->a_next)
+    SVI_REQUIRE(e->g_next && e->row_stats && e->ld_an >= N && e->ld_an % 8 == 0 &&
+                    (reinterpret_cast<uintptr_t>(e->a_next) & 15) == 0 && (reinterpret_cast<uintptr_t>(e->g_next) & 7) == 0,
+                "%s: a_next needs g_next, row_stats, ld_an >= N (multiple of 8) and 16-byte alignment", fn);
+
+  int rc = make_tmap_2d(ta, A, 2, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, BK, BM);
+  if (rc) return rc;
+  if (e->w_e4m3)   // the converters swizzle; the staging tile is plain 64-byte rows
+    rc = make_tmap_2d(tb, W, 1, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, BK, BN, /*swizzle_128b=*/false);
+  else
+    rc = make_tmap_2d(tb, W, 2, (uint64_t)K, (uint64_t)N, (uint64_t)ldw * 2, BK, BN);
+  if (rc) return rc;
+
+  ep->out = e->out; ep->ldo = e->ldo;
+  ep->bias = e->bias; ep->gate = e->gate; ep->residual = e->residual; ep->ldr = e->ldr;
+  ep->sumsq = e->sumsq; ep->sumsq_groups = e->sumsq_groups; ep->sumsq_group_cols = e->sumsq_group_cols;
+  ep->sumsq_parts = e->sumsq_parts;
+  ep->ln_stats = e->ln_stats; ep->ln_u = e->ln_u; ep->ln_inv_d = e->ln_dim > 0 ? 1.0f / (float)e->ln_dim : 0.f;
+  ep->ln_eps = e->ln_eps;
+  ep->a_next = reinterpret_cast<__nv_bfloat16*>(e->a_next); ep->ld_an = e->ld_an; ep->g_next = e->g_next;
+  ep->row_stats = e->row_stats;
+  return SVI_OK;
 }
 
 }  // namespace gemm
@@ -462,60 +569,47 @@ extern "C" int svi_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t 
                              int32_t N, int32_t K, const svi_gemm_epilogue* e, void* stream) {
   using namespace svi;
   using namespace svi::gemm;
-  SVI_REQUIRE(A && W && e && e->out, "svi_gemm_bf16: null pointer");
-  SVI_REQUIRE(M > 0 && N > 0 && K > 0, "svi_gemm_bf16: M,N,K must be positive (got %d,%d,%d)", M, N, K);
-  SVI_REQUIRE(K % 8 == 0 && N % 8 == 0, "svi_gemm_bf16: K and N must be multiples of 8 (K=%d N=%d)", K, N);
-  SVI_REQUIRE(lda % 8 == 0 && ldw % 8 == 0 && lda >= K && ldw >= K,
-              "svi_gemm_bf16: lda/ldw must be multiples of 8 and >= K");
-  SVI_REQUIRE(e->w_e4m3 == 0 || e->w_e4m3 == 1, "svi_gemm_bf16: w_e4m3 must be 0 (bf16 W) or 1 (e4m3 W), got %d", e->w_e4m3);
-  if (e->w_e4m3)
-    SVI_REQUIRE(K % 16 == 0 && ldw % 16 == 0,
-                "svi_gemm_bf16: e4m3 W needs K and ldw to be multiples of 16 (16-byte row pitch; K=%d ldw=%lld)", K,
-                (long long)ldw);
-  SVI_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(W) & 15) == 0,
-              "svi_gemm_bf16: A and W must be 16-byte aligned");
-  SVI_REQUIRE(e->ldo >= N && e->ldo % (e->out_is_f32 ? 4 : 8) == 0 &&
-                  (reinterpret_cast<uintptr_t>(e->out) & 15) == 0,
-              "svi_gemm_bf16: out must be 16-byte aligned with ldo >= N and 16-byte row pitch");
-  SVI_REQUIRE(e->act >= 0 && e->act <= 4, "svi_gemm_bf16: unknown activation %d", e->act);
-  if (e->residual)
-    SVI_REQUIRE(e->ldr >= N && e->ldr % 4 == 0 && (reinterpret_cast<uintptr_t>(e->residual) & 15) == 0,
-                "svi_gemm_bf16: residual must be 16-byte aligned with ldr >= N, ldr %% 4 == 0");
-  if (e->bias) SVI_REQUIRE((reinterpret_cast<uintptr_t>(e->bias) & 15) == 0, "svi_gemm_bf16: bias alignment");
-  if (e->gate) SVI_REQUIRE((reinterpret_cast<uintptr_t>(e->gate) & 15) == 0, "svi_gemm_bf16: gate alignment");
-  if (e->sumsq)
-    SVI_REQUIRE(e->sumsq_groups > 0 && e->sumsq_group_cols > 0 && e->sumsq_group_cols % 32 == 0,
-                "svi_gemm_bf16: sumsq_group_cols must be a positive multiple of 32");
-  if (e->sumsq && e->sumsq_parts)
-    SVI_REQUIRE(e->sumsq_group_cols % 128 == 0 && e->sumsq_parts == e->sumsq_group_cols / 128,
-                "svi_gemm_bf16: sumsq_parts must be 0 (atomic accumulation) or sumsq_group_cols / 128 with sumsq_group_cols %% 128 == 0");
-  if (e->ln_stats)
-    SVI_REQUIRE(e->ln_u && e->ln_dim > 0 && (reinterpret_cast<uintptr_t>(e->ln_stats) & 7) == 0 &&
-                    (reinterpret_cast<uintptr_t>(e->ln_u) & 7) == 0,
-                "svi_gemm_bf16: ln fold needs ln_u (8-byte aligned), ln_dim > 0 and 8-byte aligned ln_stats");
-  if (e->a_next)
-    SVI_REQUIRE(e->g_next && e->row_stats && e->ld_an >= N && e->ld_an % 8 == 0 &&
-                    (reinterpret_cast<uintptr_t>(e->a_next) & 15) == 0 && (reinterpret_cast<uintptr_t>(e->g_next) & 7) == 0,
-                "svi_gemm_bf16: a_next needs g_next, row_stats, ld_an >= N (multiple of 8) and 16-byte alignment");
-
   CUtensorMap ta, tb;
-  int rc = make_tmap_2d(&ta, A, 2, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, BK, BM);
-  if (rc) return rc;
-  if (e->w_e4m3)   // the converters swizzle; the staging tile is plain 64-byte rows
-    rc = make_tmap_2d(&tb, W, 1, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, BK, BN, /*swizzle_128b=*/false);
-  else
-    rc = make_tmap_2d(&tb, W, 2, (uint64_t)K, (uint64_t)N, (uint64_t)ldw * 2, BK, BN);
-  if (rc) return rc;
-
   Epi ep;
-  ep.out = e->out; ep.ldo = e->ldo;
-  ep.bias = e->bias; ep.gate = e->gate; ep.residual = e->residual; ep.ldr = e->ldr;
-  ep.sumsq = e->sumsq; ep.sumsq_groups = e->sumsq_groups; ep.sumsq_group_cols = e->sumsq_group_cols; ep.sumsq_parts = e->sumsq_parts;
-  ep.ln_stats = e->ln_stats; ep.ln_u = e->ln_u; ep.ln_inv_d = e->ln_dim > 0 ? 1.0f / (float)e->ln_dim : 0.f; ep.ln_eps = e->ln_eps;
-  ep.a_next = reinterpret_cast<__nv_bfloat16*>(e->a_next); ep.ld_an = e->ld_an; ep.g_next = e->g_next; ep.row_stats = e->row_stats;
-
+  const int rc = prepare("svi_gemm_bf16", A, lda, W, ldw, M, N, K, e, &ta, &tb, &ep);
+  if (rc) return rc;
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool f32 = e->out_is_f32 != 0, fold = e->ln_stats || e->a_next;
-  return e->w_e4m3 ? launch_kind<true>(ta, tb, M, N, K, e->act, f32, fold, ep, st)
-                   : launch_kind<false>(ta, tb, M, N, K, e->act, f32, fold, ep, st);
+  const LoRAArgs<false> none{};
+  return e->w_e4m3 ? launch_kind<true>(ta, tb, M, N, K, e->act, f32, fold, ep, none, st)
+                   : launch_kind<false>(ta, tb, M, N, K, e->act, f32, fold, ep, none, st);
+}
+
+extern "C" int svi_gemm_lora_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, int32_t M, int32_t N, int32_t K,
+                                  const svi_gemm_epilogue* e, const svi_gemm_lora* lora, void* stream) {
+  using namespace svi;
+  using namespace svi::gemm;
+  CUtensorMap ta, tb;
+  Epi ep;
+  int rc = prepare("svi_gemm_lora_bf16", A, lda, W, ldw, M, N, K, e, &ta, &tb, &ep);
+  if (rc) return rc;
+  SVI_REQUIRE(lora && lora->U && lora->B, "svi_gemm_lora_bf16: null LoRA pointer");
+  SVI_REQUIRE(lora->R > 0 && lora->R % BK == 0, "svi_gemm_lora_bf16: R must be a positive multiple of 64 (got %d)", lora->R);
+  SVI_REQUIRE(lora->group_cols == 0 || (lora->group_cols > 0 && lora->group_cols % BN == 0 && N % lora->group_cols == 0),
+              "svi_gemm_lora_bf16: group_cols must be 0 or a multiple of 128 that divides N (got %d, N=%d)", lora->group_cols, N);
+  const int64_t groups = lora->group_cols ? N / lora->group_cols : 1;
+  SVI_REQUIRE((reinterpret_cast<uintptr_t>(lora->U) & 15) == 0 && (reinterpret_cast<uintptr_t>(lora->B) & 15) == 0,
+              "svi_gemm_lora_bf16: U and B must be 16-byte aligned");
+  SVI_REQUIRE(lora->ldu >= groups * lora->R && lora->ldu % 8 == 0 && lora->ldb >= lora->R && lora->ldb % 8 == 0,
+              "svi_gemm_lora_bf16: ldu must be >= groups * R and ldb >= R, both multiples of 8 (ldu=%lld ldb=%lld)",
+              (long long)lora->ldu, (long long)lora->ldb);
+  SVI_REQUIRE(e->act == SVI_ACT_NONE || e->act == SVI_ACT_GELU_TANH,
+              "svi_gemm_lora_bf16: activation %d has no LoRA kernel (none or GELU-tanh)", e->act);
+  SVI_REQUIRE(!e->ln_stats && !e->a_next, "svi_gemm_lora_bf16: the LayerNorm fold (ln_* / a_next) cannot take a LoRA segment");
+  LoRAArgs<true> la;
+  la.kb = lora->R / BK;
+  la.group_cols = lora->group_cols;
+  rc = make_tmap_2d(&la.u, lora->U, 2, (uint64_t)(groups * lora->R), (uint64_t)M, (uint64_t)lora->ldu * 2, BK, BM);
+  if (rc) return rc;
+  rc = make_tmap_2d(&la.b, lora->B, 2, (uint64_t)lora->R, (uint64_t)N, (uint64_t)lora->ldb * 2, BK, BN);
+  if (rc) return rc;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool f32 = e->out_is_f32 != 0;
+  return e->w_e4m3 ? launch_kind<true>(ta, tb, M, N, K, e->act, f32, false, ep, la, st)
+                   : launch_kind<false>(ta, tb, M, N, K, e->act, f32, false, ep, la, st);
 }

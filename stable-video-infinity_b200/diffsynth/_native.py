@@ -1,4 +1,5 @@
-"""ctypes binding of the C-ABI kernel library ``libsvi_b200.so`` (declared in ``include/svi_b200.h``).
+"""ctypes binding of the C-ABI kernel library ``libsvi_b200.so`` (declared in ``include/svi_b200.h`` and
+``include/svi_b200_lora.h``).
 
 This is the only door between the Python host code and the hand-written sm_90a kernels.  There is no
 fallback: if the shared library is missing or a call fails, a ``RuntimeError`` is raised.
@@ -47,6 +48,11 @@ class ConvDesc(_c.Structure):
         ("next_gamma", _vp), ("next_silu", _i32), ("write_f32", _i32),
         ("variant", _i32),
     ]
+
+
+class GemmLoRA(_c.Structure):
+    """Mirror of ``svi_gemm_lora`` (include/svi_b200_lora.h)."""
+    _fields_ = [("U", _vp), ("ldu", _i64), ("B", _vp), ("ldb", _i64), ("R", _i32), ("group_cols", _i32)]
 
 
 # name -> (restype, argtypes); must list every symbol the header declares (checked by tests)
@@ -104,6 +110,11 @@ SIGNATURES = {
     "svi_interp_layernorm": (_i32, [_vp, _i64, _i64, _i32, _i64, _f32, _vp, _vp, _vp, _i64, _vp]),
 }
 
+# the same for include/svi_b200_lora.h
+LORA_SIGNATURES = {
+    "svi_gemm_lora_bf16": (_i32, [_vp, _i64, _vp, _i64, _i32, _i32, _i32, _c.POINTER(GemmEpilogue), _c.POINTER(GemmLoRA), _vp]),
+}
+
 _lib = None
 
 
@@ -121,7 +132,7 @@ def load():
             f"svi_b200: native kernel library not found at {_LIB_PATH}. Build it with "
             f"`python -c 'import __graft_entry__ as g; g.build()'` (or `make`) — there is no CPU fallback.")
     lib = ctypes.CDLL(_LIB_PATH)
-    for name, (res, args) in SIGNATURES.items():
+    for name, (res, args) in (SIGNATURES | LORA_SIGNATURES).items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing: fail loudly
         fn.restype = res
         fn.argtypes = args
@@ -173,6 +184,38 @@ def gemm(a, w, out, bias=None, act=ACT_NONE, gate=None, residual=None, sumsq=Non
     w.to(torch.bfloat16); it needs K % 16 == 0 and a row stride that is a multiple of 16.
     ln = (stats f32 [M,2], u f32 [N], dim, eps): LayerNorm folded into the GEMM (consumer side, svi_gemm_epilogue);
     emit = (a_next bf16 [M,N], g_next f32 [N], row_stats f32 [M,2]): producer side."""
+    ep, lda, ldw, (M, N, K) = _gemm_args(a, w, out, bias, act, gate, residual, sumsq, sumsq_group_cols, ln, emit)
+    rc = load().svi_gemm_bf16(_ptr(a, torch.bfloat16, "a"), lda, _ptr(w, name="w"), ldw,
+                              M, N, K, ctypes.byref(ep), _stream())
+    _check(rc, "svi_gemm_bf16")
+    return out
+
+
+def gemm_lora(a, w, out, u, b, R, group_cols=0, bias=None, act=ACT_NONE, gate=None, residual=None, sumsq=None,
+              sumsq_group_cols=0, ln=None, emit=None):
+    """gemm() plus an unmerged LoRA term ahead of the epilogue (svi_gemm_lora_bf16, include/svi_b200_lora.h):
+    out = epilogue(a @ w^T + u[:, g R:(g+1) R] @ b^T) with g = column // group_cols (0: one group).  u bf16 [M, >= groups R]
+    holds alpha * x A^T (row-strided views allowed, e.g. a column offset into a wider U), b bf16 [N, >= R]; R % 64 == 0.
+    act: none or GELU-tanh; ln / emit (the LayerNorm fold) are refused by the library."""
+    ep, lda, ldw, (M, N, K) = _gemm_args(a, w, out, bias, act, gate, residual, sumsq, sumsq_group_cols, ln, emit)
+    if u.shape[0] != M or b.shape[0] != N:
+        raise RuntimeError(f"svi_b200.gemm_lora: u must have M={M} rows and b N={N} rows, got u{tuple(u.shape)} b{tuple(b.shape)}")
+    groups = N // group_cols if group_cols else 1
+    if u.shape[1] < groups * R or b.shape[1] < R:
+        raise RuntimeError(f"svi_b200.gemm_lora: u needs >= {groups} x R columns and b >= R (R={R}), got u{tuple(u.shape)} "
+                           f"b{tuple(b.shape)}")
+    lo = GemmLoRA()
+    lo.U, lo.ldu = _ptr(u, torch.bfloat16, "u"), _rowmajor(u, "u")
+    lo.B, lo.ldb = _ptr(b, torch.bfloat16, "b"), _rowmajor(b, "b")
+    lo.R, lo.group_cols = int(R), int(group_cols)
+    rc = load().svi_gemm_lora_bf16(_ptr(a, torch.bfloat16, "a"), lda, _ptr(w, name="w"), ldw, M, N, K, ctypes.byref(ep),
+                                   ctypes.byref(lo), _stream())
+    _check(rc, "svi_gemm_lora_bf16")
+    return out
+
+
+def _gemm_args(a, w, out, bias, act, gate, residual, sumsq, sumsq_group_cols, ln, emit):
+    """(epilogue, lda, ldw, (M, N, K)) of one gemm / gemm_lora call, after the host-side checks."""
     if a.dtype != torch.bfloat16:
         raise RuntimeError(f"svi_b200.gemm: a must be bf16 (only the weight may be float8_e4m3fn), got {a.dtype}")
     if w.dtype not in (torch.bfloat16, torch.float8_e4m3fn):
@@ -226,10 +269,7 @@ def gemm(a, w, out, bias=None, act=ACT_NONE, gate=None, residual=None, sumsq=Non
             raise RuntimeError("svi_b200.gemm: emit needs a_next [M,N] and contiguous row_stats [M,2]")
         ep.a_next, ep.ld_an = _ptr(a_next, torch.bfloat16, "a_next"), _rowmajor(a_next, "a_next")
         ep.g_next, ep.row_stats = _ptr(g_next, torch.float32, "g_next"), _ptr(row_stats, torch.float32, "row_stats")
-    rc = load().svi_gemm_bf16(_ptr(a, torch.bfloat16, "a"), lda, _ptr(w, name="w"), ldw,
-                              M, N, K, ctypes.byref(ep), _stream())
-    _check(rc, "svi_gemm_bf16")
-    return out
+    return ep, lda, ldw, (M, N, K)
 
 
 def attention(q, k, v, out, num_heads, scale=None, accumulate=False, workspace=None):

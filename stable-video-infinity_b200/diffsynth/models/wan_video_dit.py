@@ -201,6 +201,47 @@ class _BlockWeights:
             self.nxw, self.nxb = _f32(blk.norm_x.weight, device), _f32(blk.norm_x.bias, device)
 
 
+# The block GEMMs an unmerged LoRA adapter applies to, and the modules whose adapters each one stacks (one column group per
+# module, group_cols = d for the fused ones).
+_LORA_GEMMS = (("qkv", ("self_attn.q", "self_attn.k", "self_attn.v")), ("o", ("self_attn.o",)), ("cq", ("cross_attn.q",)),
+               ("ckv", ("cross_attn.k", "cross_attn.v")), ("co", ("cross_attn.o",)), ("f0", ("ffn.0",)), ("f2", ("ffn.2",)))
+
+
+class _LoRAStack:
+    """The active adapters of one block GEMM, stacked for svi_gemm_lora_bf16: a bf16 [groups R, K] (the down-projections),
+    b bf16 [N, R] (the up-projections), gate f32 [groups R] (each adapter's alpha on its columns).  Adapter j takes the
+    columns [off_j, off_j + r_j) of every group, r_j its largest rank among the GEMM's modules (zero rows / columns where
+    a module has a smaller rank or none); R = sum r_j rounded up to a multiple of 64 (the kernel's k-block)."""
+
+    def __init__(self, adapters, block, modules, n_out, k_in, device):
+        ranks = [max((ad[(block, m)][0].shape[0] for m in modules if (block, m) in ad), default=0) for _, ad, _ in adapters]
+        groups = len(modules)
+        self.R = (sum(ranks) + 63) // 64 * 64
+        self.group_cols = n_out // groups if groups > 1 else 0
+        gc = n_out // groups
+        a = torch.zeros(groups * self.R, k_in, dtype=torch.bfloat16)
+        b = torch.zeros(n_out, self.R, dtype=torch.bfloat16)
+        self.spans = []                               # (adapter name, first column, rank) per group
+        off = 0
+        for (name, ad, _), r in zip(adapters, ranks):
+            for g, m in enumerate(modules):
+                self.spans.append((name, g * self.R + off, r))
+                if (block, m) in ad:
+                    am, bm = ad[(block, m)]
+                    a[g * self.R + off: g * self.R + off + am.shape[0]] = am
+                    b[g * gc:(g + 1) * gc, off:off + bm.shape[1]] = bm
+            off += r
+        self.a, self.b = a.to(device), b.to(device)
+        self.gate = torch.zeros(groups * self.R, dtype=torch.float32, device=device)
+        self.set_alphas({name: alpha for name, _, alpha in adapters})
+
+    def set_alphas(self, alphas):
+        g = torch.zeros(self.gate.shape[0], dtype=torch.float32)
+        for name, c0, r in self.spans:
+            g[c0:c0 + r] = float(alphas[name])
+        self.gate.copy_(g)                            # in place: captured graphs read this buffer
+
+
 class ContextState:
     """Step-invariant conditioning of one prompt: embedded context rows and every layer's cross-attention K/V
     (reference recomputes text_embedding + K/V projections on every forward, svi_video.py:92, wan_video_dit.py:273-274)."""
@@ -288,8 +329,8 @@ class _CountingNative:
             r = fn(*a, **k)
             e1.record()
             tag = name
-            if name == "gemm":
-                tag = f"gemm M={a[0].shape[0]} N={a[1].shape[0]} K={a[1].shape[1]} {_gemm_epilogue_class(a, k)}"
+            if name in ("gemm", "gemm_lora"):
+                tag = f"{name} M={a[0].shape[0]} N={a[1].shape[0]} K={a[1].shape[1]} {_gemm_epilogue_class(a, k)}"
             elif name == "attention":
                 tag = f"attention Lq={a[0].shape[0]} Lk={a[1].shape[0]}"
             self.events.append((tag, e0, e1))
@@ -362,6 +403,54 @@ class WanDiTEngine:
         self._fold_static = None
         self.attn_events = None  # bench.py: list collecting (start, end) events around self-attention launches
         self.k = _CountingNative()  # every native launch goes through this proxy (bench.py reads the count)
+        self._lora = None           # per block {GEMM: _LoRAStack} of the model's active adapters, or None
+        self._lora_version, self._lora_alphas = 0, {}
+
+    # ------------------------------------------------------------------ unmerged LoRA adapters
+    def _sync_lora(self):
+        """Follow the model's active adapter set (WanModel.set_lora_adapters).  A new set rebuilds the LoRA stacks only
+        (the base weight copies stay) and drops the captured graphs, whose launches name the old stacks; new alphas are
+        written into the stacks' gate vectors in place, so the graphs stay valid.  Both drop the cached context K|V, which
+        the cross-attention k|v adapters change."""
+        m = self.model
+        if self._lora_version != m._lora_version:
+            adapters = [(name, m._lora_adapters[name][0], alpha) for name, alpha in m._lora_active.items()]
+            self._lora = None
+            if adapters:
+                self._lora = []
+                for i, bw in enumerate(self.blocks):
+                    ws = {"qkv": bw.w_qkv, "o": bw.w_o, "cq": bw.w_cq, "ckv": bw.w_ckv, "co": bw.w_co, "f0": bw.w_f0,
+                          "f2": bw.w_f2}
+                    stacks = {}
+                    for gname, modules in _LORA_GEMMS:
+                        if any((i, md) in ad for _, ad, _ in adapters for md in modules):
+                            w = ws[gname]
+                            stacks[gname] = _LoRAStack(adapters, i, modules, w.shape[0], w.shape[1], self.device)
+                    self._lora.append(stacks)
+            self._lora_version, self._lora_alphas = m._lora_version, dict(m._lora_active)
+            self._graphs.clear()
+            self._ctx_cache.clear()
+        elif self._lora_alphas != m._lora_active:
+            for stacks in self._lora or ():
+                for st in stacks.values():
+                    st.set_alphas(m._lora_active)
+            self._lora_alphas = dict(m._lora_active)
+            self._ctx_cache.clear()
+
+    def _lora_down(self, st, a):
+        """U = gate * (a @ st.a^T) in bf16: the scaled down-projection the LoRA segment of the GEMM consumes."""
+        u = self._buf("lora_u", (a.shape[0], st.a.shape[0]), torch.bfloat16)
+        self.k.gemm(a, st.a, u, gate=st.gate)
+        return u
+
+    def _proj(self, st, a, w, out, **kw):
+        """self.k.gemm, plus the active adapters' term when the block GEMM has a _LoRAStack `st`."""
+        if st is None:
+            return self.k.gemm(a, w, out, **kw)
+        return self.k.gemm_lora(a, w, out, self._lora_down(st, a), st.b, st.R, st.group_cols, **kw)
+
+    def _lora_of(self, i):
+        return {} if self._lora is None else self._lora[i]
 
     # ------------------------------------------------------------------ helpers
     def _buf(self, name, shape, dtype):
@@ -457,8 +546,11 @@ class WanDiTEngine:
 
     def context_state(self, context, clip_feature=None) -> ContextState:
         """Embed the prompt (and CLIP) tokens and project every layer's cross-attention K/V once."""
-        # keyed by tensor IDENTITY (weak references): a freed tensor's address may be reused by different data
-        key = (id(context), context._version, None if clip_feature is None else (id(clip_feature), clip_feature._version))
+        self._sync_lora()
+        # keyed by tensor IDENTITY (weak references): a freed tensor's address may be reused by different data; and by the
+        # adapter state the K|V were projected with
+        key = (id(context), context._version, None if clip_feature is None else (id(clip_feature), clip_feature._version),
+               self._lora_version, tuple(self._lora_alphas.items()))
         hit = self._ctx_cache.get(key)
         if hit is not None and hit[0]() is context and (clip_feature is None or hit[1]() is clip_feature):
             self._ctx_cache.move_to_end(key)
@@ -504,6 +596,7 @@ class WanDiTEngine:
     def project_context(self, emb, n_img=0) -> ContextState:
         """Every layer's cross-attention K|V from EMBEDDED context rows (bf16 [n_img + n_txt, d]; image rows first):
         K = RMSNorm(k) * (w_k * w_q) — see _BlockWeights — and V, both bf16 (wan_video_dit.py:273-274, 296-299)."""
+        self._sync_lora()
         d, dev = self.dim, self.device
         n_txt = emb.shape[0] - n_img
         st = ContextState(n_img, n_txt, len(self.blocks), d, dev)
@@ -513,7 +606,7 @@ class WanDiTEngine:
         for li, bw in enumerate(self.blocks):
             kv = st.kv_txt[li]
             sl = ss[0, :n_txt]
-            self.k.gemm(emb[n_img:], bw.w_ckv, kv, bias=bw.b_ckv, sumsq=sl, sumsq_group_cols=d)
+            self._proj(self._lora_of(li).get("ckv"), emb[n_img:], bw.w_ckv, kv, bias=bw.b_ckv, sumsq=sl, sumsq_group_cols=d)
             self.k.rmsnorm_rope(kv[:, :d], sl, 0, bw.eps_qk, bw.cnk_q)       # K * rms * (w_k * w_q): see _BlockWeights
             if n_img:
                 kvi = st.kv_img[li]
@@ -581,6 +674,7 @@ class WanDiTEngine:
         ffn = self._buf("ffn", (L, bw.w_f0.shape[0]), torch.bfloat16)
         rs = self._row_sums(L) if row_sums is None else row_sums
         P = d // 128
+        lora = self._lora_of(i)
         # --- self attention
         if fold is None:
             self.k.layernorm_modulate(x, h, bw.eps, scale=mod[1], shift=mod[0])
@@ -590,7 +684,7 @@ class WanDiTEngine:
         ev = self.attn_events
         if sp is None:
             ss = rs[:2 * L * P].view(L, 2, P)
-            self.k.gemm(h, bw.w_qkv, qkv, bias=b_qkv, sumsq=ss, sumsq_group_cols=d, ln=ln1)
+            self._proj(lora.get("qkv"), h, bw.w_qkv, qkv, bias=b_qkv, sumsq=ss, sumsq_group_cols=d, ln=ln1)
             self.k.qk_norm_rope(qkv[:, :2 * d], ss, bw.eps_qk, bw.nq, bw.nk, cos, sin, 0)
             q, k, v = qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:]
         else:
@@ -607,13 +701,22 @@ class WanDiTEngine:
                 kvf = self._buf("kv_full", (L * sp.sp_size, 2 * d), torch.bfloat16)
                 kvl = kvf[sp.sp_rank * L:(sp.sp_rank + 1) * L]
             ssq, ssk = rs[:L * P].view(L, 1, P), rs[L * P:2 * L * P].view(L, 1, P)
-            self.k.gemm(h, bw.w_kv, kvl, bias=b_qkv[d:], sumsq=ssk, sumsq_group_cols=d,
-                        ln=None if ln1 is None else (ln1[0], ln1[1][d:], d, bw.eps))
+            sl = lora.get("qkv")          # U [L, 3R] holds the q | k | v groups: the two launches take their columns of it
+            u = None if sl is None else self._lora_down(sl, h)
+            if u is None:
+                self.k.gemm(h, bw.w_kv, kvl, bias=b_qkv[d:], sumsq=ssk, sumsq_group_cols=d,
+                            ln=None if ln1 is None else (ln1[0], ln1[1][d:], d, bw.eps))
+            else:
+                self.k.gemm_lora(h, bw.w_kv, kvl, u[:, sl.R:], sl.b[d:], sl.R, d, bias=b_qkv[d:], sumsq=ssk,
+                                 sumsq_group_cols=d)
             self.k.rmsnorm_rope(kvl[:, :d], ssk, 0, bw.eps_qk, bw.nk, cos, sin, sp.sp_rank * L)
             if pe is not None:
                 pe.push(pbuf)
-            self.k.gemm(h, bw.w_q, q, bias=b_qkv[:d], sumsq=ssq, sumsq_group_cols=d,
-                        ln=None if ln1 is None else (ln1[0], ln1[1][:d], d, bw.eps))
+            if u is None:
+                self.k.gemm(h, bw.w_q, q, bias=b_qkv[:d], sumsq=ssq, sumsq_group_cols=d,
+                            ln=None if ln1 is None else (ln1[0], ln1[1][:d], d, bw.eps))
+            else:
+                self.k.gemm_lora(h, bw.w_q, q, u[:, :sl.R], sl.b[:d], sl.R, 0, bias=b_qkv[:d], sumsq=ssq, sumsq_group_cols=d)
             self.k.rmsnorm_rope(q, ssq, 0, bw.eps_qk, bw.nq, cos, sin, sp.sp_rank * L)
             if pe is None:
                 sp.all_gather_rows(kvf)
@@ -630,15 +733,15 @@ class WanDiTEngine:
             e1 = torch.cuda.Event(enable_timing=True)
             e1.record()
             ev.append((e0, e1))
-        self.k.gemm(att, bw.w_o, x, bias=bw.b_o, gate=mod[2], residual=x,
-                    emit=None if fold is None else (h, bw.n3w, fold.stats[i, 1]))
+        self._proj(lora.get("o"), att, bw.w_o, x, bias=bw.b_o, gate=mod[2], residual=x,
+                   emit=None if fold is None else (h, bw.n3w, fold.stats[i, 1]))
         # --- cross attention: q stays un-normalised in memory; its RMS factor is applied inside the softmax and norm_q's
         #     weight already sits in the context K (context_state)
         cq = qkv[:, :d]
         ss1 = rs[2 * L * P:].view(L, 1, P)
         if fold is None:
             self.k.layernorm_modulate(x, h, bw.eps, gamma=bw.n3w, beta=bw.n3b)
-            self.k.gemm(h, bw.w_cq, cq, bias=bw.b_cq, sumsq=ss1, sumsq_group_cols=d)
+            self._proj(lora.get("cq"), h, bw.w_cq, cq, bias=bw.b_cq, sumsq=ss1, sumsq_group_cols=d)
         else:
             self.k.gemm(h, bw.w_cq, cq, bias=fold.c2[i], sumsq=ss1, sumsq_group_cols=d,
                         ln=(fold.stats[i, 1], fold.u2[i], d, bw.eps))
@@ -647,8 +750,8 @@ class WanDiTEngine:
         if ctx.n_img:
             kvi = ctx.kv_img[i]
             self.k.attention_qscale(cq, kvi[:, :d], kvi[:, d:], att, H, ss1, d, bw.eps_qk, accumulate=True)
-        self.k.gemm(att, bw.w_co, x, bias=bw.b_co, residual=x,
-                    emit=None if fold is None else (h, fold.v.g[i, 1], fold.stats[i, 2]))
+        self._proj(lora.get("co"), att, bw.w_co, x, bias=bw.b_co, residual=x,
+                   emit=None if fold is None else (h, fold.v.g[i, 1], fold.stats[i, 2]))
         # --- audio cross-attention (SVI-Talk, wan_video_dit.py:361-366): tokens of latent frame f attend to that frame's
         #     audio tokens (models/attention.py:318-371); 1/sqrt(head_dim) scale, no q/k norm
         if audio is not None:
@@ -668,8 +771,8 @@ class WanDiTEngine:
         # --- FFN
         if fold is None:
             self.k.layernorm_modulate(x, h, bw.eps, scale=mod[4], shift=mod[3])
-            self.k.gemm(h, bw.w_f0, ffn, bias=bw.b_f0, act=nv.ACT_GELU_TANH)
-            self.k.gemm(ffn, bw.w_f2, x, bias=bw.b_f2, gate=mod[5], residual=x)
+            self._proj(lora.get("f0"), h, bw.w_f0, ffn, bias=bw.b_f0, act=nv.ACT_GELU_TANH)
+            self._proj(lora.get("f2"), ffn, bw.w_f2, x, bias=bw.b_f2, gate=mod[5], residual=x)
         else:
             self.k.gemm(h, bw.w_f0, ffn, bias=fold.v.c3[i], act=nv.ACT_GELU_TANH, ln=(fold.stats[i, 2], fold.v.u3[i], d, bw.eps))
             last = i + 1 == len(self.blocks)
@@ -700,6 +803,7 @@ class WanDiTEngine:
             raise RuntimeError("svi_b200: channel count does not match patch_embedding")
         hh, ww = Hl // 2, Wl // 2
         L = f * hh * ww
+        self._sync_lora()
         ts = self.time_state(timestep)
         ctx = context if isinstance(context, ContextState) else self.context_state(context, clip_feature)
         cos, sin = self.rope(f, hh, ww)
@@ -785,7 +889,7 @@ class WanDiTEngine:
             cond_l = cond if sp is None else cond[sp.row_offset: sp.row_offset + Ll]
         nl = len(self.blocks)
         fold = None
-        if self.use_fold and ts.fold is not None and audio is None:
+        if self.use_fold and ts.fold is not None and audio is None and self._lora is None:   # the LoRA GEMMs take no fold
             u2, c2 = self._fold_consts()
             fold = _FoldRun(ts.fold, u2, c2, self._buf("ln_stats", (nl, 3, Ll, 2), torch.float32))
             self.k.zero_(fold.stats)
@@ -845,6 +949,47 @@ class WanModel(nn.Module):
                                              norm_output_audio=True)
         self._engine: Optional[WanDiTEngine] = None
         self._sig_params = None
+        # unmerged LoRA adapters (plain attributes, not parameters or buffers: state_dict and the fingerprints ignore them)
+        self._lora_adapters = {}      # name -> ({(block, module): (A bf16 [r, in], B bf16 [out, r])}, default alpha)
+        self._lora_active = {}        # name -> alpha, in stacking order
+        self._lora_version = 0        # bumped when the active set or an active adapter's weights change
+
+    # -- unmerged LoRA adapters ----------------------------------------------------------------
+    def add_lora_adapter(self, name, state_dict, alpha=1.0):
+        """Register a LoRA (peft keys, as ModelManager.load_lora_v2 takes them) under `name` without merging it: it runs as
+        a second K segment of the block GEMMs once set_lora_adapters activates it.  Targets: q, k, v, o of the self- and
+        cross-attention and ffn.0 / ffn.2 of every block; anything else raises ValueError (merge those with load_lora_v2).
+        The factors are kept in bf16 on the CPU; `alpha` is the scale set_lora_adapters uses when given names only."""
+        from .lora import adapter_weights
+        self._lora_adapters[name] = (adapter_weights(self, state_dict), float(alpha))
+        if name in self._lora_active:
+            self._lora_version += 1
+
+    def set_lora_adapters(self, adapters):
+        """The active adapters: {name: alpha, ...} (stacked in this order, ranks concatenated, like several LoRA files
+        merged one after the other), a list of names (each at its add_lora_adapter alpha), or {} / None for none.  Changing
+        only the alphas keeps the captured CUDA graphs of the engine."""
+        if adapters is None:
+            adapters = {}
+        elif isinstance(adapters, str):
+            adapters = [adapters]
+        if not isinstance(adapters, dict):
+            adapters = {n: self._lora_adapters[n][1] if n in self._lora_adapters else 0.0 for n in adapters}
+        unknown = [n for n in adapters if n not in self._lora_adapters]
+        if unknown:
+            raise ValueError(f"unknown LoRA adapter(s) {unknown}; loaded: {sorted(self._lora_adapters)}")
+        new = {n: float(a) for n, a in adapters.items()}
+        if list(new) != list(self._lora_active):
+            self._lora_version += 1
+        self._lora_active = new
+
+    def delete_lora_adapter(self, name):
+        """Forget an adapter (and deactivate it)."""
+        if name not in self._lora_adapters:
+            raise ValueError(f"unknown LoRA adapter {name!r}")
+        del self._lora_adapters[name]
+        if name in self._lora_active:
+            self.set_lora_adapters({n: a for n, a in self._lora_active.items() if n != name})
 
     # -- engine management -------------------------------------------------------------------
     def _param_signature(self):

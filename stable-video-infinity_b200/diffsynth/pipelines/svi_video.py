@@ -192,6 +192,31 @@ class SVIVideoPipeline(BasePipeline):
     def denoising_model(self):
         return self.dit
 
+    # ------------------------------------------------------------------ unmerged LoRA adapters
+    def load_lora_adapter(self, file_path="", adapter_name="default", lora_alpha=1.0, state_dict=None):
+        """Load an SVI LoRA (shot, film, tom, dance, talk) as a switchable adapter of the DiT and make it the only active
+        one.  Takes what ModelManager.load_lora_v2 takes: a file, a list of files whose keys are gathered, or a state dict,
+        with 'pipe.dit.'-prefixed or plain peft keys.  Unlike load_lora_v2 nothing is merged: set_lora_adapters switches
+        to another adapter, a mix or none without reloading the model, and on an FP8 model the adapter keeps bf16
+        precision.  A file that also carries other modules (the SVI-Dance pose stem, ...) raises ValueError: load those
+        with load_lora_v2."""
+        from ..models.utils import load_state_dict
+        if state_dict is None:
+            paths = file_path if isinstance(file_path, (list, tuple)) else [file_path]
+            state_dict = {}
+            for fp in paths:
+                state_dict.update(load_state_dict(fp))
+        sd = {(k.split("pipe.dit.", 1)[1] if "pipe.dit." in k else k): v for k, v in state_dict.items()}
+        self.dit.add_lora_adapter(adapter_name, sd, lora_alpha)
+        self.dit.set_lora_adapters({adapter_name: lora_alpha})
+
+    def set_lora_adapters(self, adapters):
+        """Active DiT adapters: {name: alpha, ...}, a list of names, or {} / None for the base model (WanModel.set_lora_adapters)."""
+        self.dit.set_lora_adapters(adapters)
+
+    def delete_lora_adapter(self, adapter_name):
+        self.dit.delete_lora_adapter(adapter_name)
+
     def prepare_unified_sequence_parallel(self):
         return {"use_unified_sequence_parallel": self.use_unified_sequence_parallel}
 
