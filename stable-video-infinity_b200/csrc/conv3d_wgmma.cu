@@ -13,9 +13,14 @@
 // wan_video_vae.py:153-156), fp32 NHWC out — and, fused, the NEXT conv's input: RMS_norm + SiLU (:55-70, 206-210) of the
 // output pixel (its whole channel vector sits in one accumulator row) written as bf16 straight into the next conv's frame
 // ring, so the activation between the two convs of a ResidualBlock never exists in fp32 and no staging pass runs.
+//
+// The same mainloop, instantiated with RifeParams, runs the 2-D convolutions of RIFE's IFNet (svi_rife_conv2d,
+// include/svi_b200_rife.h): "frames" are the N images of a batch (no slot table, no cap on N), and the epilogue is
+// bias -> PReLU -> + residual with the output columns split into sub-pixel phases and an optional space-to-depth bf16 copy.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "../../include/svi_b200.h"
+#include "../../include/svi_b200_rife.h"
 
 namespace svi {
 namespace conv {
@@ -56,6 +61,29 @@ struct Params {
   int next_silu;
   int write_f32;               // 0: the fp32 output is not needed (only the normalised bf16 is consumed)
 };
+
+// svi_rife_conv2d: the mainloop fields of Params, then the epilogue of svi_rife_conv_desc.  T = images, kt = 1.
+struct RifeParams {
+  int H, W, T;
+  int kt, kh, kw;
+  int pad_h, pad_w;
+  int cin_chunks;
+  int C_out, BW, BH;
+  int stages, stage_bytes;
+  int phase_cols, up;          // up = 2: four phases, destination grid 2H x 2W
+  const float* bias;
+  const float* prelu;
+  const float* residual;
+  float* out;
+  long long out_img_stride;
+  int out_ld;
+  __nv_bfloat16* out_bf;
+  long long bf_img_stride;
+  int bf_ld, bf_s2d;
+};
+
+__device__ __forceinline__ int input_slot(const Params& p, int t, int a) { return p.slot[t][a]; }
+__device__ __forceinline__ int input_slot(const RifeParams&, int t, int) { return t; }
 
 __device__ __forceinline__ void tma_load_4d_a(uint32_t smem_dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2,
                                               int c3) {
@@ -143,10 +171,58 @@ __device__ __forceinline__ void epilogue(const Params& p, float (&acc)[BN / 2], 
   }
 }
 
+// RIFE epilogue of the same slice: v = acc + bias -> PReLU -> + residual; column n = q * phase_cols + c goes to channel c
+// of destination pixel (up * y + q / 2, up * x + q % 2).  phase_cols is even, so the pair (n, n + 1) stays in one phase.
 template <int BN>
+__device__ __forceinline__ void epilogue(const RifeParams& p, float (&acc)[BN / 2], int t, int h0, int w0, int r0, int col0,
+                                         int lane) {
+  const int g = lane >> 2, c = lane & 3;
+  const int Wd = p.W * p.up;
+  int yy[2], xx[2];
+  bool ok[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = r0 + g + 8 * h;
+    yy[h] = h0 + r / p.BW;
+    xx[h] = w0 + r % p.BW;
+    ok[h] = yy[h] < p.H && xx[h] < p.W;
+  }
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int n = col0 + 8 * j + 2 * c;
+    if (n < p.C_out) {
+      const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+      const float2 a = p.prelu ? __ldg(reinterpret_cast<const float2*>(p.prelu + n)) : make_float2(1.f, 1.f);
+      const int q = n / p.phase_cols, ch = n - q * p.phase_cols;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!ok[h]) continue;
+        const int Y = yy[h] * p.up + (q >> 1), X = xx[h] * p.up + (q & 1);
+        float v0 = acc[4 * j + 2 * h] + b.x, v1 = acc[4 * j + 2 * h + 1] + b.y;
+        v0 = v0 > 0.f ? v0 : v0 * a.x;
+        v1 = v1 > 0.f ? v1 : v1 * a.y;
+        const long long o = (long long)t * p.out_img_stride + ((long long)Y * Wd + X) * p.out_ld + ch;
+        if (p.residual) {
+          const float2 r = *reinterpret_cast<const float2*>(p.residual + o);
+          v0 += r.x; v1 += r.y;
+        }
+        if (p.out) *reinterpret_cast<float2*>(p.out + o) = make_float2(v0, v1);
+        if (p.out_bf) {
+          const long long ob = p.bf_s2d
+              ? (long long)t * p.bf_img_stride + ((long long)(Y >> 1) * (Wd >> 1) + (X >> 1)) * p.bf_ld +
+                    ((Y & 1) * 2 + (X & 1)) * p.phase_cols + ch
+              : (long long)t * p.bf_img_stride + ((long long)Y * Wd + X) * p.bf_ld + ch;
+          *reinterpret_cast<uint32_t*>(p.out_bf + ob) = pack_bf16x2(v0, v1);
+        }
+      }
+    }
+  }
+}
+
+template <int BN, class P>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-            const __grid_constant__ Params p) {
+            const __grid_constant__ P p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bars = sbase + RING_BYTES;
@@ -197,7 +273,7 @@ conv_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ 
         decode_tile(tile, t, h0, w0, n_blk);
         int kcol = 0;
         for (int a = 0; a < p.kt; ++a) {
-          const int slot = p.slot[t][a];
+          const int slot = input_slot(p, t, a);
           for (int b = 0; b < p.kh; ++b) {
             for (int c = 0; c < p.kw; ++c) {
               for (int cc = 0; cc < p.cin_chunks; ++cc) {
@@ -260,13 +336,13 @@ void* encode_tiled_fn() {
   return fn;
 }
 
-template <int BN>
-int launch(const CUtensorMap& tx, const CUtensorMap& tw, Params p, int tiles, cudaStream_t stream) {
+template <int BN, class P>
+int launch(const CUtensorMap& tx, const CUtensorMap& tw, P p, int tiles, cudaStream_t stream, const char* name) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t ce = cudaFuncSetAttribute(conv_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    cudaError_t ce = cudaFuncSetAttribute(conv_kernel<BN, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (ce != cudaSuccess) {
-      set_last_error("svi_conv3d_causal: cudaFuncSetAttribute failed: %s", cudaGetErrorString(ce));
+      set_last_error("%s: cudaFuncSetAttribute failed: %s", name, cudaGetErrorString(ce));
       return SVI_ERR_LAUNCH;
     }
     attr_set = true;
@@ -276,8 +352,30 @@ int launch(const CUtensorMap& tx, const CUtensorMap& tw, Params p, int tiles, cu
   if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
   const int sms = sm_count();
   if (sms <= 0) return SVI_ERR_DRIVER;
-  conv_kernel<BN><<<tiles < sms ? tiles : sms, NUM_THREADS, SMEM_BYTES, stream>>>(tx, tw, p);
-  SVI_CUDA_LAUNCH_CHECK("svi_conv3d_causal");
+  conv_kernel<BN, P><<<tiles < sms ? tiles : sms, NUM_THREADS, SMEM_BYTES, stream>>>(tx, tw, p);
+  SVI_CUDA_LAUNCH_CHECK(name);
+  return SVI_OK;
+}
+
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+// 4-D tensor map of a channels-last bf16 stack [images][H][W][C] with 64-channel x BW x BH x 1 boxes (OOB = zero).
+int encode_input_map(CUtensorMap* tx, const void* base, int C, int W, int H, int images, int BW, int BH, const char* name) {
+  EncodeTiledFn enc = reinterpret_cast<EncodeTiledFn>(encode_tiled_fn());
+  if (!enc) return SVI_ERR_DRIVER;
+  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)images};
+  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  cuuint32_t box[4] = {BK, (cuuint32_t)BW, (cuuint32_t)BH, 1};
+  cuuint32_t es[4] = {1, 1, 1, 1};
+  CUresult r = enc(tx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, es,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_last_error("%s: input tensor map failed (CUresult %d) C=%d W=%d H=%d images=%d", name, (int)r, C, W, H, images);
+    return SVI_ERR_DRIVER;
+  }
   return SVI_OK;
 }
 
@@ -374,40 +472,99 @@ extern "C" int svi_conv3d_causal(const svi_conv_desc* d, void* stream) {
     for (int t = 0; t < d->T; ++t) SVI_REQUIRE(d->next_slot[t] >= 0, "svi_conv3d_causal: next_slot must be >= 0");
   }
 
-  typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  EncodeTiledFn enc = reinterpret_cast<EncodeTiledFn>(encode_tiled_fn());
-  if (!enc) return SVI_ERR_DRIVER;
   const int BW = d->tile_w, BH = BM / BW;
   CUtensorMap tx, tw;
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)d->C_in, (cuuint64_t)d->in_W, (cuuint64_t)d->in_H, (cuuint64_t)d->ring_slots};
-    cuuint64_t strides[3] = {(cuuint64_t)d->C_in * 2, (cuuint64_t)d->in_W * d->C_in * 2,
-                             (cuuint64_t)d->in_H * d->in_W * d->C_in * 2};
-    cuuint32_t box[4] = {BK, (cuuint32_t)BW, (cuuint32_t)BH, 1};
-    cuuint32_t es[4] = {1, 1, 1, 1};
-    CUresult r = enc(&tx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(d->x_ring), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      set_last_error("svi_conv3d_causal: input tensor map failed (CUresult %d) C=%d W=%d H=%d slots=%d", (int)r, d->C_in,
-                     d->in_W, d->in_H, d->ring_slots);
-      return SVI_ERR_DRIVER;
-    }
-  }
-  int rc = make_tmap_2d(&tw, d->w_packed, 2, (uint64_t)ktot, (uint64_t)d->w_rows, (uint64_t)d->w_ld * 2, BK, BN);
+  int rc = encode_input_map(&tx, d->x_ring, d->C_in, d->in_W, d->in_H, d->ring_slots, BW, BH, "svi_conv3d_causal");
+  if (rc) return rc;
+  rc = make_tmap_2d(&tw, d->w_packed, 2, (uint64_t)ktot, (uint64_t)d->w_rows, (uint64_t)d->w_ld * 2, BK, BN);
   if (rc) return rc;
 
   const int tiles = d->T * ((d->H + BH - 1) / BH) * ((d->W + BW - 1) / BW) * ((d->C_out + BN - 1) / BN);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const char* nm = "svi_conv3d_causal";
   switch (BN) {
-    case 16: return launch<16>(tx, tw, p, tiles, st);
-    case 32: return launch<32>(tx, tw, p, tiles, st);
-    case 64: return launch<64>(tx, tw, p, tiles, st);
-    case 96: return launch<96>(tx, tw, p, tiles, st);
-    case 128: return launch<128>(tx, tw, p, tiles, st);
-    case 192: return launch<192>(tx, tw, p, tiles, st);
-    default: return launch<256>(tx, tw, p, tiles, st);
+    case 16: return launch<16>(tx, tw, p, tiles, st, nm);
+    case 32: return launch<32>(tx, tw, p, tiles, st, nm);
+    case 64: return launch<64>(tx, tw, p, tiles, st, nm);
+    case 96: return launch<96>(tx, tw, p, tiles, st, nm);
+    case 128: return launch<128>(tx, tw, p, tiles, st, nm);
+    case 192: return launch<192>(tx, tw, p, tiles, st, nm);
+    default: return launch<256>(tx, tw, p, tiles, st, nm);
+  }
+}
+
+extern "C" int svi_rife_conv2d(const svi_rife_conv_desc* d, void* stream) {
+  using namespace svi;
+  using namespace svi::conv;
+  SVI_REQUIRE(d && d->x && d->w_packed && d->bias && (d->out || d->out_bf16), "svi_rife_conv2d: null pointer");
+  SVI_REQUIRE(d->N > 0 && d->H > 0 && d->W > 0 && d->in_H > 0 && d->in_W > 0, "svi_rife_conv2d: N, H, W, in_H, in_W must be > 0");
+  SVI_REQUIRE(d->kh >= 1 && d->kh <= 3 && d->kw >= 1 && d->kw <= 3, "svi_rife_conv2d: kernel extents must be in [1,3]");
+  SVI_REQUIRE(d->pad_h >= 0 && d->pad_h < d->kh && d->pad_w >= 0 && d->pad_w < d->kw, "svi_rife_conv2d: need 0 <= pad < extent");
+  SVI_REQUIRE(d->C_in > 0 && d->C_in % 8 == 0, "svi_rife_conv2d: C_in must be a multiple of 8 (got %d)", d->C_in);
+  SVI_REQUIRE((reinterpret_cast<uintptr_t>(d->x) & 15) == 0 && (reinterpret_cast<uintptr_t>(d->w_packed) & 15) == 0,
+              "svi_rife_conv2d: x and w_packed must be 16-byte aligned");
+  SVI_REQUIRE(d->phase_cols > 0 && d->phase_cols % 2 == 0 && d->C_out > 0 && d->C_out % d->phase_cols == 0 &&
+                  (d->C_out / d->phase_cols == 1 || d->C_out / d->phase_cols == 4),
+              "svi_rife_conv2d: phase_cols must be even and C_out must be 1 or 4 phases of it (C_out %d, phase_cols %d)",
+              d->C_out, d->phase_cols);
+  SVI_REQUIRE(d->tile_w == 8 || d->tile_w == 16 || d->tile_w == 32 || d->tile_w == 64 || d->tile_w == 128,
+              "svi_rife_conv2d: tile_w must be 8, 16, 32, 64 or 128");
+  const int cin_chunks = (d->C_in + BK - 1) / BK;
+  const int ktot = d->kh * d->kw * cin_chunks * BK;
+  SVI_REQUIRE(d->w_rows >= d->C_out && d->w_ld >= ktot && d->w_ld % 8 == 0,
+              "svi_rife_conv2d: packed weight needs >= C_out rows and ld >= kh*kw*ceil64(C_in), ld %% 8 == 0");
+  SVI_REQUIRE((reinterpret_cast<uintptr_t>(d->bias) & 7) == 0 && (reinterpret_cast<uintptr_t>(d->prelu) & 7) == 0,
+              "svi_rife_conv2d: bias and prelu must be 8-byte aligned");
+  const int up = d->C_out / d->phase_cols == 4 ? 2 : 1;
+  if (d->out || d->residual) {
+    SVI_REQUIRE((reinterpret_cast<uintptr_t>(d->out) & 7) == 0 && (reinterpret_cast<uintptr_t>(d->residual) & 7) == 0,
+                "svi_rife_conv2d: out and residual must be 8-byte aligned");
+    SVI_REQUIRE(d->out_ld % 2 == 0 && d->out_ld >= d->phase_cols && d->out_img_stride % 2 == 0 &&
+                    d->out_img_stride >= (long long)d->H * up * d->W * up * d->out_ld,
+                "svi_rife_conv2d: out_ld must be even and >= phase_cols, out_img_stride even and >= one image");
+  }
+  if (d->out_bf16) {
+    SVI_REQUIRE((reinterpret_cast<uintptr_t>(d->out_bf16) & 3) == 0, "svi_rife_conv2d: out_bf16 must be 4-byte aligned");
+    SVI_REQUIRE(d->bf_s2d == 0 || d->bf_s2d == 1, "svi_rife_conv2d: bf_s2d must be 0 or 1");
+    SVI_REQUIRE(!d->bf_s2d || ((d->H * up) % 2 == 0 && (d->W * up) % 2 == 0),
+                "svi_rife_conv2d: a space-to-depth copy needs an even destination grid");
+    const int need = d->bf_s2d ? 4 * d->phase_cols : d->phase_cols;
+    SVI_REQUIRE(d->bf_ld % 2 == 0 && d->bf_ld >= need && d->bf_img_stride % 2 == 0 &&
+                    d->bf_img_stride >= (long long)d->H * up * d->W * up / (d->bf_s2d ? 4 : 1) * d->bf_ld,
+                "svi_rife_conv2d: bf_ld must be even and hold every channel of a pixel, bf_img_stride even and >= one image");
+  }
+  // N tiles: as few as the widest instantiated width (192) allows, then the smallest width that covers each
+  const int n_tiles = (d->C_out + 191) / 192;
+  const int per = (d->C_out + n_tiles - 1) / n_tiles;
+  const int BN = per <= 32 ? 32 : per <= 64 ? 64 : per <= 96 ? 96 : 192;
+  const int BW = d->tile_w, BH = BM / BW;
+  const long long tiles = (long long)d->N * ((d->H + BH - 1) / BH) * ((d->W + BW - 1) / BW) * ((d->C_out + BN - 1) / BN);
+  SVI_REQUIRE(tiles < (1LL << 31), "svi_rife_conv2d: too many tiles in one launch (%lld)", tiles);
+
+  RifeParams p;
+  p.H = d->H; p.W = d->W; p.T = d->N;
+  p.kt = 1; p.kh = d->kh; p.kw = d->kw;
+  p.pad_h = d->pad_h; p.pad_w = d->pad_w;
+  p.cin_chunks = cin_chunks;
+  p.C_out = d->C_out; p.BW = BW; p.BH = BH;
+  p.stages = p.stage_bytes = 0;
+  p.phase_cols = d->phase_cols; p.up = up;
+  p.bias = d->bias; p.prelu = d->prelu; p.residual = d->residual;
+  p.out = d->out; p.out_img_stride = d->out_img_stride; p.out_ld = d->out_ld;
+  p.out_bf = reinterpret_cast<__nv_bfloat16*>(d->out_bf16); p.bf_img_stride = d->bf_img_stride;
+  p.bf_ld = d->bf_ld; p.bf_s2d = d->bf_s2d;
+
+  CUtensorMap tx, tw;
+  int rc = encode_input_map(&tx, d->x, d->C_in, d->in_W, d->in_H, d->N, BW, BH, "svi_rife_conv2d");
+  if (rc) return rc;
+  rc = make_tmap_2d(&tw, d->w_packed, 2, (uint64_t)ktot, (uint64_t)d->w_rows, (uint64_t)d->w_ld * 2, BK, BN);
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const char* nm = "svi_rife_conv2d";
+  switch (BN) {
+    case 32: return launch<32>(tx, tw, p, (int)tiles, st, nm);
+    case 64: return launch<64>(tx, tw, p, (int)tiles, st, nm);
+    case 96: return launch<96>(tx, tw, p, (int)tiles, st, nm);
+    default: return launch<192>(tx, tw, p, (int)tiles, st, nm);
   }
 }

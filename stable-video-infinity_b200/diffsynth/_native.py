@@ -1,5 +1,5 @@
-"""ctypes binding of the C-ABI kernel library ``libsvi_b200.so`` (declared in ``include/svi_b200.h`` and
-``include/svi_b200_lora.h``).
+"""ctypes binding of the C-ABI kernel library ``libsvi_b200.so`` (declared in ``include/svi_b200.h``,
+``include/svi_b200_lora.h`` and ``include/svi_b200_rife.h``).
 
 This is the only door between the Python host code and the hand-written sm_90a kernels.  There is no
 fallback: if the shared library is missing or a call fails, a ``RuntimeError`` is raised.
@@ -115,6 +115,50 @@ LORA_SIGNATURES = {
     "svi_gemm_lora_bf16": (_i32, [_vp, _i64, _vp, _i64, _i32, _i32, _i32, _c.POINTER(GemmEpilogue), _c.POINTER(GemmLoRA), _vp]),
 }
 
+
+class RifeConvDesc(_c.Structure):
+    """Mirror of ``svi_rife_conv_desc`` (include/svi_b200_rife.h)."""
+    _fields_ = [
+        ("x", _vp), ("N", _i32), ("in_H", _i32), ("in_W", _i32), ("C_in", _i32),
+        ("w_packed", _vp), ("w_rows", _i32), ("w_ld", _i64),
+        ("kh", _i32), ("kw", _i32), ("pad_h", _i32), ("pad_w", _i32),
+        ("H", _i32), ("W", _i32), ("C_out", _i32), ("phase_cols", _i32), ("tile_w", _i32),
+        ("bias", _vp), ("prelu", _vp), ("residual", _vp),
+        ("out", _vp), ("out_img_stride", _i64), ("out_ld", _i32),
+        ("out_bf16", _vp), ("bf_img_stride", _i64), ("bf_ld", _i32), ("bf_s2d", _i32),
+    ]
+
+
+class RifeBlockInput(_c.Structure):
+    """Mirror of ``svi_rife_block_input`` (include/svi_b200_rife.h)."""
+    _fields_ = [
+        ("img0", _vp), ("img1", _vp), ("img_stride", _i64), ("state", _vp),
+        ("pairs", _i32), ("H", _i32), ("W", _i32), ("h", _i32), ("w", _i32),
+        ("src_scale", _f32), ("flow_mul", _f32), ("out", _vp),
+    ]
+
+
+class RifeUpdate(_c.Structure):
+    """Mirror of ``svi_rife_update`` (include/svi_b200_rife.h)."""
+    _fields_ = [
+        ("heads", _vp), ("heads_ld", _i32),
+        ("pairs", _i32), ("H", _i32), ("W", _i32), ("h", _i32), ("w", _i32),
+        ("src_scale", _f32), ("flow_mul", _f32),
+        ("img0", _vp), ("img1", _vp), ("img_stride", _i64),
+        ("state", _vp), ("first", _i32),
+        ("merged", _vp), ("merged_stride", _i64), ("clip", _i32),
+        ("rgb", _vp), ("rgb_stride", _i64),
+    ]
+
+
+# the same for include/svi_b200_rife.h
+RIFE_SIGNATURES = {
+    "svi_rife_stage_frames": (_i32, [_vp, _i64, _vp, _vp]),
+    "svi_rife_block_input_launch": (_i32, [_c.POINTER(RifeBlockInput), _vp]),
+    "svi_rife_conv2d": (_i32, [_c.POINTER(RifeConvDesc), _vp]),
+    "svi_rife_update_warp": (_i32, [_c.POINTER(RifeUpdate), _vp]),
+}
+
 _lib = None
 
 
@@ -132,7 +176,7 @@ def load():
             f"svi_b200: native kernel library not found at {_LIB_PATH}. Build it with "
             f"`python -c 'import __graft_entry__ as g; g.build()'` (or `make`) — there is no CPU fallback.")
     lib = ctypes.CDLL(_LIB_PATH)
-    for name, (res, args) in (SIGNATURES | LORA_SIGNATURES).items():
+    for name, (res, args) in (SIGNATURES | LORA_SIGNATURES | RIFE_SIGNATURES).items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing: fail loudly
         fn.restype = res
         fn.argtypes = args
@@ -720,3 +764,105 @@ def interp_layernorm(x, T_out, gamma, beta, eps, out):
                                      _ptr(out, torch.bfloat16, "out"), _rowmajor(out, "out"), _stream())
     _check(rc, "svi_interp_layernorm")
     return out
+
+
+# --------------------------------------------------------------------------------------------- RIFE (include/svi_b200_rife.h)
+def _contig(t, dtype, name):
+    if t is None:
+        return None
+    if not t.is_contiguous():
+        raise RuntimeError(f"svi_b200: {name} must be contiguous")
+    return _ptr(t, dtype, name)
+
+
+def _frames_view(t, name, C):
+    """(pointer, stride between frames) of an f32 / uint8 [n, H, W, C] view whose frames are each contiguous."""
+    n, H, W, c = t.shape
+    if c != C or t.stride()[1:] != (W * C, C, 1):
+        raise RuntimeError(f"svi_b200: {name} must be [n, H, W, {C}] with contiguous frames, got {tuple(t.shape)} / {t.stride()}")
+    return t.stride(0)
+
+
+def rife_stage_frames(rgb, out):
+    """out f32 [n, H, W, 4] = B, G, R, 0 of uint8 rgb [n, H, W, 3] / 255 (svi_rife_stage_frames)."""
+    if rgb.dtype != torch.uint8 or rgb.shape[-1] != 3 or out.shape[-1] != 4 or rgb.numel() // 3 != out.numel() // 4:
+        raise RuntimeError("svi_b200.rife_stage_frames: rgb must be uint8 [..., 3] and out f32 [..., 4] of as many pixels")
+    _check(load().svi_rife_stage_frames(_contig(rgb, torch.uint8, "rgb"), rgb.numel() // 3, _contig(out, torch.float32, "out"),
+                                        _stream()), "svi_rife_stage_frames")
+    return out
+
+
+def rife_block_input(img0, img1, state, h, w, src_scale, flow_mul, out):
+    """out bf16 [2 pairs, h/2, w/2, 48]: both directions' space-to-depth block input (svi_rife_block_input_launch).
+    img0 / img1 f32 [pairs, H, W, 4] views sharing one frame stride; state f32 [pairs, H, W, 12] or None (first block)."""
+    P, H, W, _ = img0.shape
+    s0, s1 = _frames_view(img0, "img0", 4), _frames_view(img1, "img1", 4)
+    if img1.shape != img0.shape or s0 != s1 or tuple(out.shape) != (2 * P, h // 2, w // 2, 48):
+        raise RuntimeError("svi_b200.rife_block_input: img0 / img1 must match and out must be [2 pairs, h/2, w/2, 48]")
+    if state is not None and tuple(state.shape) != (P, H, W, 12):
+        raise RuntimeError("svi_b200.rife_block_input: state must be [pairs, H, W, 12]")
+    d = RifeBlockInput()
+    d.img0, d.img1, d.img_stride = _ptr(img0, torch.float32, "img0"), _ptr(img1, torch.float32, "img1"), s0
+    d.state = _contig(state, torch.float32, "state")
+    d.pairs, d.H, d.W, d.h, d.w = P, H, W, int(h), int(w)
+    d.src_scale, d.flow_mul = float(src_scale), float(flow_mul)
+    d.out = _contig(out, torch.bfloat16, "out")
+    _check(load().svi_rife_block_input_launch(ctypes.byref(d), _stream()), "svi_rife_block_input_launch")
+    return out
+
+
+def rife_conv2d(x, w, kh, kw, pad, C_out, phase_cols, bias, tile_w, prelu=None, residual=None, out=None, out_bf16=None,
+                bf_s2d=False):
+    """svi_rife_conv2d on x bf16 [N, H, W, C_in] (output grid H x W, stride 1, top / left padding `pad`) with the packed
+    weight w bf16 [>= C_out, >= kh kw ceil64(C_in)]: v = x * w + bias -> PReLU (prelu [C_out] or None) -> + residual.
+    With C_out = 4 phase_cols the columns are the 2 x 2 sub-pixel phases of a destination grid 2H x 2W.
+    out f32 [N, Hd, Wd, out_ld]; out_bf16 bf16 [N, Hd, Wd, bf_ld] or, with bf_s2d, [N, Hd/2, Wd/2, bf_ld] space-to-depth."""
+    N, H, W, C_in = x.shape
+    d = RifeConvDesc()
+    d.x, d.N, d.in_H, d.in_W, d.C_in = _contig(x, torch.bfloat16, "x"), N, H, W, C_in
+    d.w_packed, d.w_rows, d.w_ld = _ptr(w, torch.bfloat16, "w"), w.shape[0], _rowmajor(w, "w")
+    d.kh, d.kw, d.pad_h, d.pad_w, d.H, d.W = kh, kw, pad, pad, H, W
+    d.C_out, d.phase_cols, d.tile_w = C_out, phase_cols, tile_w
+    if bias.numel() < C_out or (prelu is not None and prelu.numel() < C_out):
+        raise RuntimeError("svi_b200.rife_conv2d: bias and prelu need C_out entries")
+    d.bias, d.prelu = _contig(bias, torch.float32, "bias"), _contig(prelu, torch.float32, "prelu")
+    lay = out if out is not None else residual
+    if residual is not None and out is not None and residual.shape != out.shape:
+        raise RuntimeError("svi_b200.rife_conv2d: residual must have the shape of out")
+    if lay is not None:
+        if lay.dim() != 4 or lay.shape[0] != N:
+            raise RuntimeError("svi_b200.rife_conv2d: out / residual must be [N, Hd, Wd, out_ld]")
+        d.out_img_stride, d.out_ld = lay[0].numel(), lay.shape[3]
+    d.residual, d.out = _contig(residual, torch.float32, "residual"), _contig(out, torch.float32, "out")
+    if out_bf16 is not None:
+        if out_bf16.dim() != 4 or out_bf16.shape[0] != N:
+            raise RuntimeError("svi_b200.rife_conv2d: out_bf16 must be [N, ., ., bf_ld]")
+        d.out_bf16, d.bf_img_stride, d.bf_ld = _contig(out_bf16, torch.bfloat16, "out_bf16"), out_bf16[0].numel(), out_bf16.shape[3]
+        d.bf_s2d = int(bool(bf_s2d))
+    _check(load().svi_rife_conv2d(ctypes.byref(d), _stream()), "svi_rife_conv2d")
+
+
+def rife_update_warp(heads, src_scale, flow_mul, img0, img1, state, first, merged=None, clip=False, rgb=None):
+    """svi_rife_update_warp: heads f32 [2 pairs, h, w, ld] -> state f32 [pairs, H, W, 12] (updated in place); merged f32
+    [pairs, H, W, 4] view (B, G, R blend, sigmoid(mask)) and rgb uint8 [pairs, H, W, 3] view, each optional."""
+    P, H, W, _ = img0.shape
+    s0, s1 = _frames_view(img0, "img0", 4), _frames_view(img1, "img1", 4)
+    if img1.shape != img0.shape or s0 != s1 or heads.shape[0] != 2 * P or tuple(state.shape) != (P, H, W, 12):
+        raise RuntimeError("svi_b200.rife_update_warp: img0 / img1 [pairs, H, W, 4], heads [2 pairs, h, w, ld] and state "
+                           "[pairs, H, W, 12] required")
+    d = RifeUpdate()
+    d.heads, d.heads_ld = _contig(heads, torch.float32, "heads"), heads.shape[3]
+    d.pairs, d.H, d.W, d.h, d.w = P, H, W, heads.shape[1], heads.shape[2]
+    d.src_scale, d.flow_mul = float(src_scale), float(flow_mul)
+    d.img0, d.img1, d.img_stride = _ptr(img0, torch.float32, "img0"), _ptr(img1, torch.float32, "img1"), s0
+    d.state, d.first = _contig(state, torch.float32, "state"), int(bool(first))
+    if merged is not None:
+        if merged.shape[0] != P:
+            raise RuntimeError("svi_b200.rife_update_warp: merged must have one frame per pair")
+        d.merged, d.merged_stride = _ptr(merged, torch.float32, "merged"), _frames_view(merged, "merged", 4)
+    d.clip = int(bool(clip))
+    if rgb is not None:
+        if rgb.shape[0] != P:
+            raise RuntimeError("svi_b200.rife_update_warp: rgb must have one frame per pair")
+        d.rgb, d.rgb_stride = _ptr(rgb, torch.uint8, "rgb"), _frames_view(rgb, "rgb", 3)
+    _check(load().svi_rife_update_warp(ctypes.byref(d), _stream()), "svi_rife_update_warp")

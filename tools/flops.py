@@ -33,3 +33,14 @@ def vae_encode_flops(t_lat, H, W):
 def vae_min_bytes(t_lat, h, w):
     """Minimal conv in+out traffic (bf16) of the VAE decoder per clip: 8.5 GB per latent frame at 480p (60x104), SURVEY §8d."""
     return 8.5e9 * t_lat * (h * w) / 6240.0
+
+
+def rife_interp_flops(H, W, scale=1.0):
+    """Algorithmic FLOPs of one interpolated frame (RIFE IFNet, 3 blocks x 2 directions; torch.utils.flop_counter's count
+    on the reference module): 102.4 GFLOP at 832x480, 236.3 GFLOP at 1280x720 (scale 1)."""
+    tot = 0.0
+    for s in (4 / scale, 2 / scale, 1 / scale):
+        p2, p4 = (H / s) * (W / s) / 4, (H / s) * (W / s) / 16
+        macs = p2 * 45 * 11 * 9 + p4 * 90 * 45 * 9 + 8 * p4 * 90 * 90 * 9 + 2 * p4 * 90 * 45 * 16 + p2 * 45 * (4 + 1) * 16
+        tot += 2 * 2 * macs
+    return tot
