@@ -17,9 +17,14 @@
 // The same mainloop, instantiated with RifeParams, runs the 2-D convolutions of RIFE's IFNet (svi_rife_conv2d,
 // include/svi_b200_rife.h): "frames" are the N images of a batch (no slot table, no cap on N), and the epilogue is
 // bias -> PReLU -> + residual with the output columns split into sub-pixel phases and an optional space-to-depth bf16 copy.
+//
+// A third instantiation, with EsrganParams, runs ESRGAN's RRDBNet (svi_esrgan_conv2d, include/svi_b200_esrgan.h): the
+// input map reads a channel prefix [0, C_in) of a wider pixel (pitch in_ld), and the epilogue is bias -> LeakyReLU -> up to
+// two scaled residuals, with f32, bf16 (channel offset, optional nearest x2) and uint8 RGB outputs.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "../../include/svi_b200.h"
+#include "../../include/svi_b200_esrgan.h"
 #include "../../include/svi_b200_rife.h"
 
 namespace svi {
@@ -82,8 +87,30 @@ struct RifeParams {
   int bf_ld, bf_s2d;
 };
 
+// svi_esrgan_conv2d: the mainloop fields of Params, then the epilogue of svi_esrgan_conv_desc.  T = images, kt = 1.
+struct EsrganParams {
+  int H, W, T;
+  int kt, kh, kw;
+  int pad_h, pad_w;
+  int cin_chunks;
+  int C_out, BW, BH;
+  int stages, stage_bytes;
+  const float* bias;
+  float slope;                 // 0: no activation
+  const float* residual;
+  float res_scale;
+  const float* residual2;
+  float res2_scale;
+  float* out;                  // f32 [T][H][W][f_ld]; residual and residual2 share the layout
+  int f_ld;
+  __nv_bfloat16* out_bf;       // bf16 [T][up H][up W][bf_ld]
+  int bf_ld, bf_up2;
+  uint8_t* out_u8;             // uint8 [T][H][W][3]
+};
+
 __device__ __forceinline__ int input_slot(const Params& p, int t, int a) { return p.slot[t][a]; }
 __device__ __forceinline__ int input_slot(const RifeParams&, int t, int) { return t; }
+__device__ __forceinline__ int input_slot(const EsrganParams&, int t, int) { return t; }
 
 __device__ __forceinline__ void tma_load_4d_a(uint32_t smem_dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2,
                                               int c3) {
@@ -213,6 +240,67 @@ __device__ __forceinline__ void epilogue(const RifeParams& p, float (&acc)[BN / 
                     ((Y & 1) * 2 + (X & 1)) * p.phase_cols + ch
               : (long long)t * p.bf_img_stride + ((long long)Y * Wd + X) * p.bf_ld + ch;
           *reinterpret_cast<uint32_t*>(p.out_bf + ob) = pack_bf16x2(v0, v1);
+        }
+      }
+    }
+  }
+}
+
+// ESRGAN epilogue of the same slice, in the reference's op order with every step rounded on its own (__fmul_rn /
+// __fadd_rn keep ptxas from contracting the residual steps into FMAs).  The pair (n, n + 1) is one 4-byte bf16 store.
+template <int BN>
+__device__ __forceinline__ void epilogue(const EsrganParams& p, float (&acc)[BN / 2], int t, int h0, int w0, int r0,
+                                         int col0, int lane) {
+  const int g = lane >> 2, c = lane & 3;
+  const int up = p.bf_up2 ? 2 : 1;
+  const int Wd = p.W * up;
+  int yy[2], xx[2];
+  bool ok[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = r0 + g + 8 * h;
+    yy[h] = h0 + r / p.BW;
+    xx[h] = w0 + r % p.BW;
+    ok[h] = yy[h] < p.H && xx[h] < p.W;
+  }
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int n = col0 + 8 * j + 2 * c;
+    if (n < p.C_out) {
+      const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!ok[h]) continue;
+        const long long pix = ((long long)t * p.H + yy[h]) * p.W + xx[h];
+        const long long o = pix * p.f_ld + n;
+        float v0 = __fadd_rn(acc[4 * j + 2 * h], b.x), v1 = __fadd_rn(acc[4 * j + 2 * h + 1], b.y);
+        if (p.slope != 0.f) {
+          v0 = v0 > 0.f ? v0 : __fmul_rn(v0, p.slope);
+          v1 = v1 > 0.f ? v1 : __fmul_rn(v1, p.slope);
+        }
+        if (p.residual) {
+          const float2 r = *reinterpret_cast<const float2*>(p.residual + o);
+          v0 = __fadd_rn(__fmul_rn(v0, p.res_scale), r.x);
+          v1 = __fadd_rn(__fmul_rn(v1, p.res_scale), r.y);
+        }
+        if (p.residual2) {
+          const float2 r = *reinterpret_cast<const float2*>(p.residual2 + o);
+          v0 = __fadd_rn(__fmul_rn(v0, p.res2_scale), r.x);
+          v1 = __fadd_rn(__fmul_rn(v1, p.res2_scale), r.y);
+        }
+        if (p.out) *reinterpret_cast<float2*>(p.out + o) = make_float2(v0, v1);
+        if (p.out_bf) {
+          const uint32_t pk = pack_bf16x2(v0, v1);
+          const long long img = (long long)t * p.H * up;
+          for (int dy = 0; dy < up; ++dy)
+            for (int dx = 0; dx < up; ++dx)
+              *reinterpret_cast<uint32_t*>(
+                  p.out_bf + ((img + yy[h] * up + dy) * Wd + xx[h] * up + dx) * p.bf_ld + n) = pk;
+        }
+        if (p.out_u8) {
+          uint8_t* q = p.out_u8 + pix * 3;
+          if (n < 3) q[n] = (uint8_t)fminf(fmaxf(__fmul_rn(v0, 255.f), 0.f), 255.f);
+          if (n + 1 < 3) q[n + 1] = (uint8_t)fminf(fmaxf(__fmul_rn(v1, 255.f), 0.f), 255.f);
         }
       }
     }
@@ -361,12 +449,14 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-// 4-D tensor map of a channels-last bf16 stack [images][H][W][C] with 64-channel x BW x BH x 1 boxes (OOB = zero).
-int encode_input_map(CUtensorMap* tx, const void* base, int C, int W, int H, int images, int BW, int BH, const char* name) {
+// 4-D tensor map of channels [0, C) of a channels-last bf16 stack [images][H][W][ld] with 64-channel x BW x BH x 1 boxes
+// (OOB = zero: channels C .. ceil64(C) read as zero even where the pixel holds more channels).
+int encode_input_map(CUtensorMap* tx, const void* base, int C, int ld, int W, int H, int images, int BW, int BH,
+                     const char* name) {
   EncodeTiledFn enc = reinterpret_cast<EncodeTiledFn>(encode_tiled_fn());
   if (!enc) return SVI_ERR_DRIVER;
   cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)images};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  cuuint64_t strides[3] = {(cuuint64_t)ld * 2, (cuuint64_t)W * ld * 2, (cuuint64_t)H * W * ld * 2};
   cuuint32_t box[4] = {BK, (cuuint32_t)BW, (cuuint32_t)BH, 1};
   cuuint32_t es[4] = {1, 1, 1, 1};
   CUresult r = enc(tx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, es,
@@ -474,7 +564,7 @@ extern "C" int svi_conv3d_causal(const svi_conv_desc* d, void* stream) {
 
   const int BW = d->tile_w, BH = BM / BW;
   CUtensorMap tx, tw;
-  int rc = encode_input_map(&tx, d->x_ring, d->C_in, d->in_W, d->in_H, d->ring_slots, BW, BH, "svi_conv3d_causal");
+  int rc = encode_input_map(&tx, d->x_ring, d->C_in, d->C_in, d->in_W, d->in_H, d->ring_slots, BW, BH, "svi_conv3d_causal");
   if (rc) return rc;
   rc = make_tmap_2d(&tw, d->w_packed, 2, (uint64_t)ktot, (uint64_t)d->w_rows, (uint64_t)d->w_ld * 2, BK, BN);
   if (rc) return rc;
@@ -555,7 +645,7 @@ extern "C" int svi_rife_conv2d(const svi_rife_conv_desc* d, void* stream) {
   p.bf_ld = d->bf_ld; p.bf_s2d = d->bf_s2d;
 
   CUtensorMap tx, tw;
-  int rc = encode_input_map(&tx, d->x, d->C_in, d->in_W, d->in_H, d->N, BW, BH, "svi_rife_conv2d");
+  int rc = encode_input_map(&tx, d->x, d->C_in, d->C_in, d->in_W, d->in_H, d->N, BW, BH, "svi_rife_conv2d");
   if (rc) return rc;
   rc = make_tmap_2d(&tw, d->w_packed, 2, (uint64_t)ktot, (uint64_t)d->w_rows, (uint64_t)d->w_ld * 2, BK, BN);
   if (rc) return rc;
@@ -566,5 +656,85 @@ extern "C" int svi_rife_conv2d(const svi_rife_conv_desc* d, void* stream) {
     case 64: return launch<64>(tx, tw, p, (int)tiles, st, nm);
     case 96: return launch<96>(tx, tw, p, (int)tiles, st, nm);
     default: return launch<192>(tx, tw, p, (int)tiles, st, nm);
+  }
+}
+
+extern "C" int svi_esrgan_conv2d(const svi_esrgan_conv_desc* d, void* stream) {
+  using namespace svi;
+  using namespace svi::conv;
+  SVI_REQUIRE(d && d->x && d->w_packed && d->bias && (d->out || d->out_bf16 || d->out_u8), "svi_esrgan_conv2d: null pointer");
+  SVI_REQUIRE(d->N > 0 && d->H > 0 && d->W > 0, "svi_esrgan_conv2d: N, H, W must be > 0");
+  SVI_REQUIRE(d->C_in > 0 && d->C_in % 8 == 0 && d->in_ld % 8 == 0 && d->in_ld >= d->C_in,
+              "svi_esrgan_conv2d: need C_in %% 8 == 0, in_ld %% 8 == 0 and in_ld >= C_in (got C_in %d, in_ld %d)", d->C_in,
+              d->in_ld);
+  SVI_REQUIRE((reinterpret_cast<uintptr_t>(d->x) & 15) == 0 && (reinterpret_cast<uintptr_t>(d->w_packed) & 15) == 0,
+              "svi_esrgan_conv2d: x and w_packed must be 16-byte aligned");
+  SVI_REQUIRE(d->C_out > 0 && d->C_out % 2 == 0, "svi_esrgan_conv2d: C_out must be even and > 0 (got %d)", d->C_out);
+  SVI_REQUIRE(d->tile_w == 8 || d->tile_w == 16 || d->tile_w == 32 || d->tile_w == 64 || d->tile_w == 128,
+              "svi_esrgan_conv2d: tile_w must be 8, 16, 32, 64 or 128");
+  const int cin_chunks = (d->C_in + BK - 1) / BK;
+  const int ktot = 9 * cin_chunks * BK;
+  SVI_REQUIRE(d->w_rows >= d->C_out && d->w_ld >= ktot && d->w_ld % 8 == 0,
+              "svi_esrgan_conv2d: packed weight needs >= C_out rows and ld >= 9*ceil64(C_in), ld %% 8 == 0");
+  SVI_REQUIRE((reinterpret_cast<uintptr_t>(d->bias) & 7) == 0, "svi_esrgan_conv2d: bias must be 8-byte aligned");
+  if (d->out || d->residual || d->residual2) {
+    SVI_REQUIRE(((reinterpret_cast<uintptr_t>(d->out) | reinterpret_cast<uintptr_t>(d->residual) |
+                  reinterpret_cast<uintptr_t>(d->residual2)) & 7) == 0,
+                "svi_esrgan_conv2d: out, residual and residual2 must be 8-byte aligned");
+    SVI_REQUIRE(d->f_ld % 2 == 0 && d->f_ld >= d->C_out, "svi_esrgan_conv2d: f_ld must be even and >= C_out (got %d)", d->f_ld);
+  }
+  const long long in_bytes = (long long)d->N * d->H * d->W * d->in_ld * 2;
+  if (d->out_bf16) {
+    SVI_REQUIRE((reinterpret_cast<uintptr_t>(d->out_bf16) & 3) == 0,
+                "svi_esrgan_conv2d: out_bf16 must be 4-byte aligned (an even channel offset)");
+    SVI_REQUIRE(d->bf_up2 == 0 || d->bf_up2 == 1, "svi_esrgan_conv2d: bf_up2 must be 0 or 1");
+    SVI_REQUIRE(d->bf_ld % 2 == 0 && d->bf_ld >= d->C_out, "svi_esrgan_conv2d: bf_ld must be even and >= C_out (got %d)",
+                d->bf_ld);
+    // The launch reads channels [0, C_in) of x while it writes: a destination in x's buffer must keep x's pixel layout
+    // and lie past the read window, or a tile would read channels another tile is writing.
+    const int up = d->bf_up2 ? 2 : 1;
+    const long long out_bytes = (long long)d->N * d->H * up * d->W * up * d->bf_ld * 2;
+    const char* xb = static_cast<const char*>(d->x);
+    const char* ob = static_cast<const char*>(d->out_bf16);
+    if (ob < xb + in_bytes && xb < ob + out_bytes) {
+      SVI_REQUIRE(ob >= xb && !d->bf_up2 && d->bf_ld == d->in_ld,
+                  "svi_esrgan_conv2d: a bf16 destination that overlaps x must lie in x's buffer with its pixel layout");
+      const long long ch = (long long)(ob - xb) / 2 % d->in_ld;
+      SVI_REQUIRE(ch >= d->C_in && ch + d->C_out <= d->in_ld,
+                  "svi_esrgan_conv2d: the bf16 destination (channels %lld..%lld) lies inside the input's read window "
+                  "[0, %d)", ch, ch + d->C_out, d->C_in);
+    }
+  }
+  SVI_REQUIRE(!d->out_u8 || d->C_out >= 3, "svi_esrgan_conv2d: a uint8 RGB output needs C_out >= 3");
+  const int BN = d->C_out <= 16 ? 16 : d->C_out <= 32 ? 32 : 64;
+  const int BW = d->tile_w, BH = BM / BW;
+  const long long tiles = (long long)d->N * ((d->H + BH - 1) / BH) * ((d->W + BW - 1) / BW) * ((d->C_out + BN - 1) / BN);
+  SVI_REQUIRE(tiles < (1LL << 31), "svi_esrgan_conv2d: too many tiles in one launch (%lld)", tiles);
+
+  EsrganParams p;
+  p.H = d->H; p.W = d->W; p.T = d->N;
+  p.kt = 1; p.kh = 3; p.kw = 3;
+  p.pad_h = 1; p.pad_w = 1;
+  p.cin_chunks = cin_chunks;
+  p.C_out = d->C_out; p.BW = BW; p.BH = BH;
+  p.stages = p.stage_bytes = 0;
+  p.bias = d->bias; p.slope = d->slope;
+  p.residual = d->residual; p.res_scale = d->res_scale;
+  p.residual2 = d->residual2; p.res2_scale = d->res2_scale;
+  p.out = d->out; p.f_ld = d->f_ld;
+  p.out_bf = reinterpret_cast<__nv_bfloat16*>(d->out_bf16); p.bf_ld = d->bf_ld; p.bf_up2 = d->bf_up2;
+  p.out_u8 = d->out_u8;
+
+  CUtensorMap tx, tw;
+  int rc = encode_input_map(&tx, d->x, d->C_in, d->in_ld, d->W, d->H, d->N, BW, BH, "svi_esrgan_conv2d");
+  if (rc) return rc;
+  rc = make_tmap_2d(&tw, d->w_packed, 2, (uint64_t)ktot, (uint64_t)d->w_rows, (uint64_t)d->w_ld * 2, BK, BN);
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const char* nm = "svi_esrgan_conv2d";
+  switch (BN) {
+    case 16: return launch<16>(tx, tw, p, (int)tiles, st, nm);
+    case 32: return launch<32>(tx, tw, p, (int)tiles, st, nm);
+    default: return launch<64>(tx, tw, p, (int)tiles, st, nm);
   }
 }

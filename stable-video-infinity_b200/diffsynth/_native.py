@@ -1,5 +1,5 @@
 """ctypes binding of the C-ABI kernel library ``libsvi_b200.so`` (declared in ``include/svi_b200.h``,
-``include/svi_b200_lora.h`` and ``include/svi_b200_rife.h``).
+``include/svi_b200_lora.h``, ``include/svi_b200_rife.h`` and ``include/svi_b200_esrgan.h``).
 
 This is the only door between the Python host code and the hand-written sm_90a kernels.  There is no
 fallback: if the shared library is missing or a call fails, a ``RuntimeError`` is raised.
@@ -159,6 +159,27 @@ RIFE_SIGNATURES = {
     "svi_rife_update_warp": (_i32, [_c.POINTER(RifeUpdate), _vp]),
 }
 
+
+class EsrganConvDesc(_c.Structure):
+    """Mirror of ``svi_esrgan_conv_desc`` (include/svi_b200_esrgan.h)."""
+    _fields_ = [
+        ("x", _vp), ("N", _i32), ("H", _i32), ("W", _i32), ("C_in", _i32), ("in_ld", _i32),
+        ("w_packed", _vp), ("w_rows", _i32), ("w_ld", _i64),
+        ("C_out", _i32), ("tile_w", _i32),
+        ("bias", _vp), ("slope", _f32),
+        ("residual", _vp), ("res_scale", _f32), ("residual2", _vp), ("res2_scale", _f32),
+        ("out", _vp), ("f_ld", _i32),
+        ("out_bf16", _vp), ("bf_ld", _i32), ("bf_up2", _i32),
+        ("out_u8", _vp),
+    ]
+
+
+# the same for include/svi_b200_esrgan.h
+ESRGAN_SIGNATURES = {
+    "svi_esrgan_stage_frames": (_i32, [_vp, _i64, _vp, _vp]),
+    "svi_esrgan_conv2d": (_i32, [_c.POINTER(EsrganConvDesc), _vp]),
+}
+
 _lib = None
 
 
@@ -176,7 +197,7 @@ def load():
             f"svi_b200: native kernel library not found at {_LIB_PATH}. Build it with "
             f"`python -c 'import __graft_entry__ as g; g.build()'` (or `make`) — there is no CPU fallback.")
     lib = ctypes.CDLL(_LIB_PATH)
-    for name, (res, args) in (SIGNATURES | LORA_SIGNATURES | RIFE_SIGNATURES).items():
+    for name, (res, args) in (SIGNATURES | LORA_SIGNATURES | RIFE_SIGNATURES | ESRGAN_SIGNATURES).items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing: fail loudly
         fn.restype = res
         fn.argtypes = args
@@ -866,3 +887,60 @@ def rife_update_warp(heads, src_scale, flow_mul, img0, img1, state, first, merge
             raise RuntimeError("svi_b200.rife_update_warp: rgb must have one frame per pair")
         d.rgb, d.rgb_stride = _ptr(rgb, torch.uint8, "rgb"), _frames_view(rgb, "rgb", 3)
     _check(load().svi_rife_update_warp(ctypes.byref(d), _stream()), "svi_rife_update_warp")
+
+
+# --------------------------------------------------------------------------------------------- ESRGAN (include/svi_b200_esrgan.h)
+def esrgan_stage_frames(rgb, out):
+    """out bf16 [n, H, W, 8] = bf16(R, G, B / 255), 0 x 5 of uint8 rgb [n, H, W, 3] (svi_esrgan_stage_frames)."""
+    if rgb.dtype != torch.uint8 or rgb.shape[-1] != 3 or out.shape[-1] != 8 or rgb.numel() // 3 != out.numel() // 8:
+        raise RuntimeError("svi_b200.esrgan_stage_frames: rgb must be uint8 [..., 3] and out bf16 [..., 8] of as many pixels")
+    _check(load().svi_esrgan_stage_frames(_contig(rgb, torch.uint8, "rgb"), rgb.numel() // 3,
+                                          _contig(out, torch.bfloat16, "out"), _stream()), "svi_esrgan_stage_frames")
+    return out
+
+
+def _channel_window(t, name):
+    """(pointer, pitch) of a bf16 [N, H, W, c] view that is a channel window of a contiguous [N, H, W, pitch] buffer."""
+    N, H, W, c = t.shape
+    ld = t.stride(2)
+    if t.stride(3) != 1 or ld < c or t.stride(1) != W * ld or t.stride(0) != H * W * ld:
+        raise RuntimeError(f"svi_b200: {name} must be a channel window of a contiguous [N, H, W, pitch] buffer, got "
+                           f"{tuple(t.shape)} / {t.stride()}")
+    return _ptr(t, torch.bfloat16, name), ld
+
+
+def esrgan_conv2d(x, w, C_out, bias, tile_w, slope=0.0, residual=None, res_scale=1.0, residual2=None, res2_scale=1.0,
+                  out=None, out_bf16=None, bf_up2=False, out_u8=None):
+    """svi_esrgan_conv2d: a 3x3, stride-1, padding-1 convolution of x (bf16 [N, H, W, C_in], a channel window x[..., :C_in]
+    of a wider buffer allowed) with the packed weight w bf16 [>= C_out, >= 9 ceil64(C_in)]:
+    v = acc + bias -> LeakyReLU(slope) -> v * res_scale + residual -> v * res2_scale + residual2.
+    out, residual, residual2 f32 [N, H, W, f_ld] (contiguous); out_bf16 bf16 [N, Hd, Wd, C_out] channel window of a
+    contiguous buffer, Hd x Wd = H x W or 2H x 2W with bf_up2; out_u8 uint8 [N, H, W, 3] (channels 0..2)."""
+    N, H, W, C_in = x.shape
+    d = EsrganConvDesc()
+    d.x, d.in_ld = _channel_window(x, "x")
+    d.N, d.H, d.W, d.C_in = N, H, W, C_in
+    d.w_packed, d.w_rows, d.w_ld = _ptr(w, torch.bfloat16, "w"), w.shape[0], _rowmajor(w, "w")
+    d.C_out, d.tile_w = C_out, tile_w
+    if bias.numel() < C_out:
+        raise RuntimeError("svi_b200.esrgan_conv2d: bias needs C_out entries")
+    d.bias, d.slope = _contig(bias, torch.float32, "bias"), float(slope)
+    f32 = [t for t in (out, residual, residual2) if t is not None]
+    if f32:
+        if any(t.shape != f32[0].shape for t in f32) or tuple(f32[0].shape[:3]) != (N, H, W):
+            raise RuntimeError("svi_b200.esrgan_conv2d: out, residual and residual2 must be [N, H, W, f_ld] of one shape")
+        d.f_ld = f32[0].shape[3]
+    d.residual, d.res_scale = _contig(residual, torch.float32, "residual"), float(res_scale)
+    d.residual2, d.res2_scale = _contig(residual2, torch.float32, "residual2"), float(res2_scale)
+    d.out = _contig(out, torch.float32, "out")
+    if out_bf16 is not None:
+        up = 2 if bf_up2 else 1
+        if tuple(out_bf16.shape) != (N, up * H, up * W, C_out):
+            raise RuntimeError(f"svi_b200.esrgan_conv2d: out_bf16 must be [N, {up}H, {up}W, C_out], got {tuple(out_bf16.shape)}")
+        d.out_bf16, d.bf_ld = _channel_window(out_bf16, "out_bf16")
+        d.bf_up2 = int(bool(bf_up2))
+    if out_u8 is not None:
+        if tuple(out_u8.shape) != (N, H, W, 3):
+            raise RuntimeError("svi_b200.esrgan_conv2d: out_u8 must be [N, H, W, 3]")
+        d.out_u8 = _contig(out_u8, torch.uint8, "out_u8")
+    _check(load().svi_esrgan_conv2d(ctypes.byref(d), _stream()), "svi_esrgan_conv2d")

@@ -1,8 +1,9 @@
 """ModelManager — checkpoint detection/loading boundary (reference diffsynth/models/model_manager.py).
 
 Only the Wan rows of the reference's hash table are kept (model_config.py:117-125); the inherited
-DiffSynth-Studio model zoo is out of scope (SURVEY.md §2 row 23), except RIFE's flownet.pkl (model_config.py:100),
-which loads as diffsynth.extensions.RIFE.IFNet.  Detection is by the md5 of the sorted
+DiffSynth-Studio model zoo is out of scope (SURVEY.md §2 row 23), except the two post-processing models: RIFE's
+flownet.pkl (model_config.py:100), which loads as diffsynth.extensions.RIFE.IFNet, and RealESRGAN_x4.pth
+(model_config.py:101), which loads as diffsynth.extensions.ESRGAN.RRDBNet.  Detection is by the md5 of the sorted
 'key[:shape]' list exactly as the reference does (models/utils.py:179-182), so real Wan2.1 checkpoints and
 SVI LoRA files resolve to the same classes.
 """
@@ -17,6 +18,7 @@ from .wan_video_dit import WanModel
 
 
 def _loader_table():
+    from ..extensions.ESRGAN import RRDBNet
     from ..extensions.RIFE import IFNet
     from .wan_video_image_encoder import WanImageEncoder
     from .wan_video_text_encoder import WanTextEncoder
@@ -33,6 +35,7 @@ def _loader_table():
         (None, "1378ea763357eea97acdef78e65d6d96", ["wan_video_vae"], [WanVideoVAE], "civitai"),
         (None, "ccc42284ea13e1ad04693284c7a09be6", ["wan_video_vae"], [WanVideoVAE], "civitai"),
         (None, "9b9313d104ac4df27991352fec013fd4", ["rife"], [IFNet], "civitai"),                # flownet.pkl, :100
+        (None, "6b7116078c4170bfbeaedc8fe71f6649", ["esrgan"], [RRDBNet], "civitai"),            # RealESRGAN_x4.pth, :101
     ]
 
 
