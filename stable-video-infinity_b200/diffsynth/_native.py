@@ -1,5 +1,6 @@
 """ctypes binding of the C-ABI kernel library ``libsvi_b200.so`` (declared in ``include/svi_b200.h``,
-``include/svi_b200_lora.h``, ``include/svi_b200_rife.h`` and ``include/svi_b200_esrgan.h``).
+``include/svi_b200_lora.h``, ``include/svi_b200_rife.h``, ``include/svi_b200_esrgan.h`` and
+``include/svi_b200_fastblend.h``).
 
 This is the only door between the Python host code and the hand-written sm_90a kernels.  There is no
 fallback: if the shared library is missing or a call fails, a ``RuntimeError`` is raised.
@@ -180,6 +181,42 @@ ESRGAN_SIGNATURES = {
     "svi_esrgan_conv2d": (_i32, [_c.POINTER(EsrganConvDesc), _vp]),
 }
 
+
+class FastblendStepDesc(_c.Structure):
+    """Mirror of ``svi_fastblend_step_desc`` (include/svi_b200_fastblend.h)."""
+    _fields_ = [
+        ("src_guide", _vp), ("src_style", _vp), ("tgt_guide", _vp), ("tgt_style", _vp),
+        ("nnf_in", _vp), ("err_in", _vp), ("nnf_out", _vp), ("err_out", _vp),
+        ("B", _i32), ("H", _i32), ("W", _i32), ("patch_size", _i32), ("mode", _i32), ("dir", _i32),
+        ("draw", _c.c_uint32), ("radius", _i32), ("guide_weight", _f32),
+    ]
+
+
+class FastblendTableDesc(_c.Structure):
+    """Mirror of ``svi_fastblend_table_desc`` (include/svi_b200_fastblend.h)."""
+    _fields_ = [
+        ("op", _i32), ("n_pix", _i64),
+        ("a", _vp), ("a_type", _i32), ("sa", _c.c_double),
+        ("b", _vp), ("b_type", _i32), ("sb", _c.c_double),
+        ("c", _vp), ("c_type", _i32), ("sc", _c.c_double),
+        ("out", _vp), ("out_type", _i32),
+    ]
+
+
+# the same for include/svi_b200_fastblend.h
+FASTBLEND_SIGNATURES = {
+    "svi_fastblend_stage_frames": (_i32, [_vp, _i64, _vp, _vp]),
+    "svi_fastblend_downsample": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "svi_fastblend_nnf_identity": (_i32, [_vp, _i32, _i32, _i32, _vp]),
+    "svi_fastblend_nnf_upscale": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp]),
+    "svi_fastblend_remap": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "svi_fastblend_step": (_i32, [_c.POINTER(FastblendStepDesc), _vp]),
+    "svi_fastblend_table": (_i32, [_c.POINTER(FastblendTableDesc), _vp]),
+}
+FB_CURRENT, FB_NEIGHBOUR, FB_RANDOM = 0, 1, 2
+FB_U8, FB_F32, FB_F64 = 0, 1, 2
+FB_MEAN, FB_HALF, FB_WSUM = 0, 1, 2
+
 _lib = None
 
 
@@ -197,7 +234,8 @@ def load():
             f"svi_b200: native kernel library not found at {_LIB_PATH}. Build it with "
             f"`python -c 'import __graft_entry__ as g; g.build()'` (or `make`) — there is no CPU fallback.")
     lib = ctypes.CDLL(_LIB_PATH)
-    for name, (res, args) in (SIGNATURES | LORA_SIGNATURES | RIFE_SIGNATURES | ESRGAN_SIGNATURES).items():
+    for name, (res, args) in (SIGNATURES | LORA_SIGNATURES | RIFE_SIGNATURES | ESRGAN_SIGNATURES |
+                        FASTBLEND_SIGNATURES).items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing: fail loudly
         fn.restype = res
         fn.argtypes = args
@@ -944,3 +982,106 @@ def esrgan_conv2d(x, w, C_out, bias, tile_w, slope=0.0, residual=None, res_scale
             raise RuntimeError("svi_b200.esrgan_conv2d: out_u8 must be [N, H, W, 3]")
         d.out_u8 = _contig(out_u8, torch.uint8, "out_u8")
     _check(load().svi_esrgan_conv2d(ctypes.byref(d), _stream()), "svi_esrgan_conv2d")
+
+
+# --------------------------------------------------------------------------------------------- FastBlend (include/svi_b200_fastblend.h)
+def _fb_frames(t, name, dtype=torch.float32, C=4):
+    if t.dim() != 4 or t.shape[-1] != C or not t.is_contiguous():
+        raise RuntimeError(f"svi_b200: {name} must be contiguous [B, H, W, {C}], got {tuple(t.shape)} / {t.stride()}")
+    return _ptr(t, dtype, name)
+
+
+def fastblend_stage_frames(rgb, out):
+    """out f32 [..., 4] = R, G, B, 0 of uint8 rgb [..., 3] (svi_fastblend_stage_frames)."""
+    if rgb.dtype != torch.uint8 or rgb.shape[-1] != 3 or out.shape[-1] != 4 or rgb.numel() // 3 != out.numel() // 4:
+        raise RuntimeError("svi_b200.fastblend_stage_frames: rgb must be uint8 [..., 3] and out f32 [..., 4] of as many pixels")
+    _check(load().svi_fastblend_stage_frames(_contig(rgb, torch.uint8, "rgb"), rgb.numel() // 3,
+                                             _contig(out, torch.float32, "out"), _stream()), "svi_fastblend_stage_frames")
+    return out
+
+
+def fastblend_downsample(src, k, out):
+    """out f32 [n, H/k, W/k, 4]: the integer-ratio INTER_AREA pyramid level of src f32 [n, H, W, 4]."""
+    n, H, W, _ = src.shape
+    if tuple(out.shape) != (n, H // k, W // k, 4):
+        raise RuntimeError("svi_b200.fastblend_downsample: out must be [n, H/k, W/k, 4]")
+    _check(load().svi_fastblend_downsample(_fb_frames(src, "src"), n, H, W, int(k), _fb_frames(out, "out"), _stream()),
+           "svi_fastblend_downsample")
+    return out
+
+
+def fastblend_nnf_identity(nnf):
+    """nnf int32 [B, H, W, 2] = (y, x)."""
+    B, H, W, _ = nnf.shape
+    _check(load().svi_fastblend_nnf_identity(_fb_frames(nnf, "nnf", torch.int32, 2), B, H, W, _stream()),
+           "svi_fastblend_nnf_identity")
+    return nnf
+
+
+def fastblend_nnf_upscale(src, out):
+    """out int32 [B, 2h, 2w, 2]: the field of an exactly doubled level from src int32 [B, h, w, 2]."""
+    B, h, w, _ = src.shape
+    if tuple(out.shape) != (B, 2 * h, 2 * w, 2):
+        raise RuntimeError("svi_b200.fastblend_nnf_upscale: out must be [B, 2h, 2w, 2]")
+    _check(load().svi_fastblend_nnf_upscale(_fb_frames(src, "src", torch.int32, 2), B, h, w,
+                                            _fb_frames(out, "out", torch.int32, 2), _stream()), "svi_fastblend_nnf_upscale")
+    return out
+
+
+def fastblend_remap(style, nnf, patch_size, out):
+    """out f32 [B, H, W, 4]: style f32 [B, H, W, 4] remapped through nnf int32 [B, H, W, 2] (svi_fastblend_remap)."""
+    B, H, W, _ = style.shape
+    if tuple(nnf.shape) != (B, H, W, 2) or out.shape != style.shape:
+        raise RuntimeError("svi_b200.fastblend_remap: style, nnf and out must describe the same [B, H, W] pixels")
+    _check(load().svi_fastblend_remap(_fb_frames(style, "style"), _fb_frames(nnf, "nnf", torch.int32, 2), B, H, W,
+                                      int(patch_size), _fb_frames(out, "out"), _stream()), "svi_fastblend_remap")
+    return out
+
+
+def fastblend_step(src_guide, src_style, tgt_guide, tgt_style, nnf_in, err_in, nnf_out, err_out, patch_size, mode,
+                   guide_weight, dir=0, draw=0, radius=0):
+    """One PatchMatch step (svi_fastblend_step): frames f32 [B, H, W, 4], fields int32 [B, H, W, 2], errors f32 [B, H, W]."""
+    B, H, W, _ = src_guide.shape
+    if any(t.shape != src_guide.shape for t in (src_style, tgt_guide, tgt_style)) or tuple(nnf_in.shape) != (B, H, W, 2) \
+            or nnf_out.shape != nnf_in.shape or tuple(err_out.shape) != (B, H, W) or (err_in is not None and err_in.shape != err_out.shape):
+        raise RuntimeError("svi_b200.fastblend_step: frames, fields and errors must describe the same [B, H, W] pixels")
+    d = FastblendStepDesc()
+    d.src_guide, d.src_style = _fb_frames(src_guide, "src_guide"), _fb_frames(src_style, "src_style")
+    d.tgt_guide, d.tgt_style = _fb_frames(tgt_guide, "tgt_guide"), _fb_frames(tgt_style, "tgt_style")
+    d.nnf_in, d.nnf_out = _fb_frames(nnf_in, "nnf_in", torch.int32, 2), _fb_frames(nnf_out, "nnf_out", torch.int32, 2)
+    d.err_in, d.err_out = _contig(err_in, torch.float32, "err_in"), _contig(err_out, torch.float32, "err_out")
+    d.B, d.H, d.W, d.patch_size, d.mode, d.dir = B, H, W, int(patch_size), int(mode), int(dir)
+    d.draw, d.radius, d.guide_weight = int(draw) & 0xFFFFFFFF, int(radius), float(guide_weight)
+    _check(load().svi_fastblend_step(ctypes.byref(d), _stream()), "svi_fastblend_step")
+
+
+_FB_TYPES = {torch.float32: FB_F32, torch.float64: FB_F64}
+
+
+def fastblend_table(op, out, a, sa=0.0, b=None, sb=0.0, c=None, sc=0.0, a_u8=False, b_u8=False, c_u8=False):
+    """svi_fastblend_table on [..., 4] frames of one pixel count.  An operand flagged `_u8` is a uint8 frame held as its f32
+    values; out is f32 / f64 [..., 4], or uint8 [..., 3] for the WSUM's clipped, truncated bytes."""
+    d = FastblendTableDesc()
+    n = a.numel() // 4
+    d.op, d.n_pix = int(op), n
+
+    def operand(t, u8, name):
+        if t.shape[-1] != 4 or t.numel() // 4 != n:
+            raise RuntimeError(f"svi_b200.fastblend_table: {name} must be [..., 4] of {n} pixels")
+        if t.dtype not in _FB_TYPES or (u8 and t.dtype != torch.float32):
+            raise RuntimeError(f"svi_b200.fastblend_table: {name} must be f32 or f64 (a uint8 frame is held as f32)")
+        return _contig(t, t.dtype, name), FB_U8 if u8 else _FB_TYPES[t.dtype]
+
+    d.a, d.a_type = operand(a, a_u8, "a")
+    d.b, d.b_type = operand(b, b_u8, "b")
+    d.sa, d.sb, d.sc = float(sa), float(sb), float(sc)
+    if c is not None:
+        d.c, d.c_type = operand(c, c_u8, "c")
+    if out.dtype == torch.uint8:
+        if out.shape[-1] != 3 or out.numel() // 3 != n:
+            raise RuntimeError("svi_b200.fastblend_table: a uint8 out must be [..., 3] of as many pixels")
+        d.out, d.out_type = _contig(out, torch.uint8, "out"), FB_U8
+    else:
+        d.out, d.out_type = operand(out, False, "out")
+    _check(load().svi_fastblend_table(ctypes.byref(d), _stream()), "svi_fastblend_table")
+    return out
