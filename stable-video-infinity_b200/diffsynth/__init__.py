@@ -8,6 +8,8 @@ _LAZY = {
     "ModelManager": ("diffsynth.models.model_manager", "ModelManager"),
     "SVIVideoPipeline": ("diffsynth.pipelines.svi_video", "SVIVideoPipeline"),
     "WanVideoPipeline": ("diffsynth.pipelines.wan_video", "WanVideoPipeline"),
+    "WanUniAnimateVideoPipeline": ("diffsynth.pipelines.wan_video", "WanUniAnimateVideoPipeline"),
+    "WanUniAnimateLongVideoPipeline": ("diffsynth.pipelines.wan_video", "WanUniAnimateLongVideoPipeline"),
     "SVIDanceVideoPipeline": ("diffsynth.pipelines.svi_video_dance", "SVIDanceVideoPipeline"),
     "SVITalkVideoPipeline": ("diffsynth.pipelines.svi_video_talk", "SVITalkVideoPipeline"),
     "save_video": ("diffsynth.data.video", "save_video"),

@@ -1,6 +1,6 @@
 """ctypes binding of the C-ABI kernel library ``libsvi_b200.so`` (declared in ``include/svi_b200.h``,
-``include/svi_b200_lora.h``, ``include/svi_b200_rife.h``, ``include/svi_b200_esrgan.h`` and
-``include/svi_b200_fastblend.h``).
+``include/svi_b200_lora.h``, ``include/svi_b200_rife.h``, ``include/svi_b200_esrgan.h``,
+``include/svi_b200_fastblend.h`` and ``include/svi_b200_unianimate.h``).
 
 This is the only door between the Python host code and the hand-written sm_90a kernels.  There is no
 fallback: if the shared library is missing or a call fails, a ``RuntimeError`` is raised.
@@ -217,6 +217,12 @@ FB_CURRENT, FB_NEIGHBOUR, FB_RANDOM = 0, 1, 2
 FB_U8, FB_F32, FB_F64 = 0, 1, 2
 FB_MEAN, FB_HALF, FB_WSUM = 0, 1, 2
 
+# the same for include/svi_b200_unianimate.h
+UNIANIMATE_SIGNATURES = {
+    "svi_window_accumulate": (_i32, [_vp, _i32, _i32, _i64, _i32, _vp, _i32, _i32, _vp]),
+    "svi_window_normalize": (_i32, [_vp, _vp, _i32, _i32, _i64, _vp, _vp]),
+}
+
 _lib = None
 
 
@@ -235,7 +241,7 @@ def load():
             f"`python -c 'import __graft_entry__ as g; g.build()'` (or `make`) — there is no CPU fallback.")
     lib = ctypes.CDLL(_LIB_PATH)
     for name, (res, args) in (SIGNATURES | LORA_SIGNATURES | RIFE_SIGNATURES | ESRGAN_SIGNATURES |
-                        FASTBLEND_SIGNATURES).items():
+                        FASTBLEND_SIGNATURES | UNIANIMATE_SIGNATURES).items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing: fail loudly
         fn.restype = res
         fn.argtypes = args
@@ -1084,4 +1090,33 @@ def fastblend_table(op, out, a, sa=0.0, b=None, sb=0.0, c=None, sc=0.0, a_u8=Fal
     else:
         d.out, d.out_type = operand(out, False, "out")
     _check(load().svi_fastblend_table(ctypes.byref(d), _stream()), "svi_fastblend_table")
+    return out
+
+
+# --------------------------------------------------------------------------------------------- UniAnimate (include/svi_b200_unianimate.h)
+def _latents_view(t, name):
+    """(C, frames, h*w) of a contiguous f32 [1, C, frames, h, w] tensor."""
+    if t.dim() != 5 or t.shape[0] != 1 or not t.is_contiguous():
+        raise RuntimeError(f"svi_b200: {name} must be a contiguous [1, C, f, h, w] tensor, got {tuple(t.shape)}")
+    return t.shape[1], t.shape[2], t.shape[3] * t.shape[4]
+
+
+def window_accumulate(win, skip, sum_, start):
+    """sum_[:, :, start + skip:start + cs] += win[:, :, skip:] (svi_window_accumulate); f32 [1, C, cs | F, h, w]."""
+    C, cs, hw = _latents_view(win, "win")
+    C2, F, hw2 = _latents_view(sum_, "sum")
+    if (C2, hw2) != (C, hw):
+        raise RuntimeError("svi_b200.window_accumulate: win and sum must have the same channels and frame size")
+    _check(load().svi_window_accumulate(_ptr(win, torch.float32, "win"), C, cs, hw, int(skip),
+                                        _ptr(sum_, torch.float32, "sum"), F, int(start), _stream()), "svi_window_accumulate")
+    return sum_
+
+
+def window_normalize(sum_, count, out):
+    """out = sum_ / count[frame] (svi_window_normalize); sum_ and out f32 [1, C, F, h, w], count int32 [F]."""
+    C, F, hw = _latents_view(sum_, "sum")
+    if _latents_view(out, "out") != (C, F, hw) or tuple(count.shape) != (F,) or not count.is_contiguous():
+        raise RuntimeError("svi_b200.window_normalize: out must match sum and count must be [F]")
+    _check(load().svi_window_normalize(_ptr(sum_, torch.float32, "sum"), _ptr(count, torch.int32, "count"), C, F, hw,
+                                       _ptr(out, torch.float32, "out"), _stream()), "svi_window_normalize")
     return out

@@ -11,6 +11,11 @@ as extra-module keys of the SVI-Dance LoRA file (``dwpose_embedding.N.{weight,bi
 (``svi_conv3d_causal`` with an explicit frame-slot table: symmetric temporal padding and temporal stride are just a
 different table; spatial stride 2 with padding 1 is a 2x2 conv over a space-to-depth input, weights repacked on the
 host), SiLU fused into the bf16 staging of the next conv's input, the final projection on ``svi_gemm_bf16``.
+
+UniAnimate-DiT adds a second, 2-D stem on a single reference-pose image (``randomref_embedding_pose``, reference
+``pipelines/wan_video.py:543-558``): six ``nn.Conv2d`` 3x3 / padding 1 (3 -> 16 -> 16 -> 16 -> 16 -> 16 -> 20 channels,
+strides 1, 1, 1, 2, 2, 2, SiLU after all but the last).  ``RandomRefEmbeddingEngine`` runs it on the same conv launch as
+the 3-D stem with one frame and kt = 1.
 """
 import torch
 import torch.nn as nn
@@ -32,14 +37,16 @@ def make_dwpose_embedding(dim=5120, concat_dim=4):
 
 
 def slot_table(frames, zero_slot, T_out, t_stride, kt):
-    """Ring slots read by output frame t, tap a: input frame t*t_stride + a - 1 (symmetric temporal padding 1), the zero
-    slot outside the video.  Pure host logic (CPU-tested against nn.Conv3d)."""
+    """Ring slots read by output frame t, tap a: input frame t*t_stride + a - (kt-1)//2 (symmetric temporal padding:
+    1 for the 3x3x3 convs, 0 for a Conv2d run as kt = 1), the zero slot outside the video.  Pure host logic (CPU-tested
+    against nn.Conv3d and nn.Conv2d)."""
     n_in = len(frames)
+    pad = (kt - 1) // 2
     table = []
     for t in range(T_out):
         row = []
         for a in range(kt):
-            i = t * t_stride + a - 1
+            i = t * t_stride + a - pad
             row.append(frames[i] if 0 <= i < n_in else zero_slot)
         table.append(row)
     return table
@@ -69,20 +76,18 @@ class StemPlan:
         self.b_proj = last.bias.detach().to(dev, torch.float32).contiguous()
 
 
-class DWPoseEmbeddingEngine:
+class _StemEngine:
+    """The conv launch both pose stems share."""
     MAX_T = 4      # output frames per conv launch (slot table of svi_conv_desc)
 
-    def __init__(self, seq: nn.Sequential, device):
-        nv.require_cuda(device, "the pose stem")
+    def __init__(self, device, what):
+        nv.require_cuda(device, what)
         self.device = torch.device(device)
-        plan = StemPlan(seq, self.device)
-        self.c, self.full, self.down, self.t_stride = plan.c, plan.full, plan.down, plan.t_stride
-        self.kproj, self.w_proj, self.b_proj = plan.kproj, plan.w_proj, plan.b_proj
         self.launches = 0
 
-    # ------------------------------------------------------------------ helpers
     def _conv(self, cv, ring, frames, T_out, t_stride, H, W):
-        """out[t] = sum_a w[a] * in[t*t_stride + a - 1] (zero outside): symmetric temporal padding 1, spatial padding 1."""
+        """out[t] = sum_a w[a] * in[t*t_stride + a - (kt-1)//2] (zero outside): symmetric temporal padding, spatial
+        padding 1."""
         full_table = slot_table(frames, ring.slots, T_out, t_stride, cv.kt)
         out = torch.empty(T_out, H, W, cv.c_out, device=self.device, dtype=torch.float32)
         for t0 in range(0, T_out, self.MAX_T):
@@ -106,6 +111,14 @@ class DWPoseEmbeddingEngine:
             nv.conv3d_causal(d)
             self.launches += 1
         return out
+
+
+class DWPoseEmbeddingEngine(_StemEngine):
+    def __init__(self, seq: nn.Sequential, device):
+        super().__init__(device, "the pose stem")
+        plan = StemPlan(seq, self.device)
+        self.c, self.full, self.down, self.t_stride = plan.c, plan.full, plan.down, plan.t_stride
+        self.kproj, self.w_proj, self.b_proj = plan.kproj, plan.w_proj, plan.b_proj
 
     def forward(self, pose):
         """pose f32 [3, T, H, W] (already /255 and front-padded as in :527) -> tokens f32 [1, f*h*w, dim]."""
@@ -164,3 +177,54 @@ def pose_condition(engine, humanpose_data):
     x = humanpose_data.to(torch.float32)
     x = torch.cat([x[:, :1].repeat(1, 3, 1, 1), x], dim=1) / 255.0
     return engine.forward(x)
+
+
+def make_randomref_embedding_pose(concat_dim=4, randomref_dim=20):
+    """The reference-pose stem of UniAnimate-DiT (reference wan_video.py:543-558), keys `0.weight` ... `10.bias`."""
+    c = concat_dim * 4
+    return nn.Sequential(
+        nn.Conv2d(3, c, 3, stride=1, padding=1), nn.SiLU(),
+        nn.Conv2d(c, c, 3, stride=1, padding=1), nn.SiLU(),
+        nn.Conv2d(c, c, 3, stride=1, padding=1), nn.SiLU(),
+        nn.Conv2d(c, c, 3, stride=2, padding=1), nn.SiLU(),
+        nn.Conv2d(c, c, 3, stride=2, padding=1), nn.SiLU(),
+        nn.Conv2d(c, randomref_dim, 3, stride=2, padding=1))
+
+
+class RandomRefEmbeddingEngine(_StemEngine):
+    """The reference-pose stem on svi_conv3d_causal: one frame, kt = 1; the stride-2 convs as 2x2 convs over a
+    space-to-depth input, SiLU fused into each conv's input staging."""
+
+    def __init__(self, seq: nn.Sequential, device):
+        super().__init__(device, "the reference-pose stem")
+        convs = [m for m in seq if isinstance(m, nn.Conv2d)]
+        if len(convs) != 6 or [m.stride[0] for m in convs] != [1, 1, 1, 2, 2, 2]:
+            raise RuntimeError("randomref_embedding_pose must be the 6-conv stem of wan_video.py:544-558")
+        self.full = [_Conv(m.weight, m.bias, self.device) for m in convs[:3]]
+        self.down = [_Conv(m.weight, m.bias, self.device, s2d="before") for m in convs[3:]]
+        self.out_channels = convs[-1].out_channels
+
+    def forward(self, image):
+        """image f32 [3, H, W] (already /255) -> f32 [1, out_channels, 1, H/8, W/8]."""
+        dev = self.device
+        C, H, W = image.shape
+        if C != 3 or H % 8 or W % 8:
+            raise RuntimeError(f"svi_b200: reference pose must be [3, H, W] with H, W multiples of 8, got {tuple(image.shape)}")
+        image = image.to(device=dev, dtype=torch.float32).contiguous()
+        ring = _Ring(1, H, W, self.full[0].c_in, dev, history=0)
+        xin = torch.empty(H, W, 8, device=dev, dtype=torch.float32)
+        nv.vae_from_planar(image, 3, H * W, None, None, xin, 8, False)
+        nv.vae_norm_act(xin, H * W, 8, 8, None, False, ring.buf[0], ring.C)
+        self.launches += 2
+        x = self._conv(self.full[0], ring, [0], 1, 1, H, W)
+        for cv in self.full[1:]:
+            nv.vae_norm_act(x[0], H * W, x.shape[-1], x[0].stride(1), None, True, ring.buf[0], ring.C)   # SiLU -> bf16
+            self.launches += 1
+            x = self._conv(cv, ring, [0], 1, 1, H, W)
+        for cv in self.down:
+            _, Hn, Wn, Cn = x.shape
+            ring = _Ring(1, Hn // 2, Wn // 2, 4 * Cn, dev, history=0)
+            nv.vae_space_to_depth_act(x[0], Hn, Wn, Cn, nv.ACT_SILU, ring.buf[0])
+            self.launches += 1
+            x = self._conv(cv, ring, [0], 1, 1, Hn // 2, Wn // 2)
+        return x[..., :self.out_channels].permute(3, 0, 1, 2).unsqueeze(0).contiguous()

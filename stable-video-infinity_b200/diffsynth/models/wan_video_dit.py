@@ -11,6 +11,7 @@ Numerics policy (SURVEY.md §7 hard part 1): bf16 GEMM/attention operands, fp32 
 stream / norms / softmax / modulation; RoPE in fp32 with an fp64-built (cos, sin) table.
 """
 import math
+import types
 import weakref
 from collections import OrderedDict
 from typing import Optional, Tuple
@@ -355,7 +356,12 @@ class WanDiTEngine:
     def __init__(self, model: "WanModel", device):
         nv.require_cuda(device, "the Wan DiT")
         self.device = torch.device(device)
-        self.model = model
+        # what the engine reads from the model, held here rather than through the model: the model caches its engine
+        # (WanModel._engine), so a reference back would be a cycle that keeps every weight copy on the device alive after
+        # the model is dropped, until Python's cyclic garbage collector happens to run
+        self.freq_dim = model.freq_dim
+        self.has_image_input, self.enable_multitalk = model.has_image_input, getattr(model, "enable_multitalk", False)
+        self._lora_state = model._lora_state
         self.dim, self.H = model.dim, model.num_heads
         self.sig = model._param_signature()
         d = self.dim
@@ -412,9 +418,9 @@ class WanDiTEngine:
         (the base weight copies stay) and drops the captured graphs, whose launches name the old stacks; new alphas are
         written into the stacks' gate vectors in place, so the graphs stay valid.  Both drop the cached context K|V, which
         the cross-attention k|v adapters change."""
-        m = self.model
-        if self._lora_version != m._lora_version:
-            adapters = [(name, m._lora_adapters[name][0], alpha) for name, alpha in m._lora_active.items()]
+        m = self._lora_state
+        if self._lora_version != m.version:
+            adapters = [(name, m.adapters[name][0], alpha) for name, alpha in m.active.items()]
             self._lora = None
             if adapters:
                 self._lora = []
@@ -427,14 +433,14 @@ class WanDiTEngine:
                             w = ws[gname]
                             stacks[gname] = _LoRAStack(adapters, i, modules, w.shape[0], w.shape[1], self.device)
                     self._lora.append(stacks)
-            self._lora_version, self._lora_alphas = m._lora_version, dict(m._lora_active)
+            self._lora_version, self._lora_alphas = m.version, dict(m.active)
             self._graphs.clear()
             self._ctx_cache.clear()
-        elif self._lora_alphas != m._lora_active:
+        elif self._lora_alphas != m.active:
             for stacks in self._lora or ():
                 for st in stacks.values():
-                    st.set_alphas(m._lora_active)
-            self._lora_alphas = dict(m._lora_active)
+                    st.set_alphas(m.active)
+            self._lora_alphas = dict(m.active)
             self._ctx_cache.clear()
 
     def _lora_down(self, st, a):
@@ -464,7 +470,7 @@ class WanDiTEngine:
     def rope(self, f, h, w):
         key = (f, h, w)
         if key not in self._rope:
-            self._rope[key] = rope_table(self.model.freqs, f, h, w, self.device)
+            self._rope[key] = rope_table(precompute_freqs_cis_3d(self.dim // self.H), f, h, w, self.device)
         return self._rope[key]
 
     # ------------------------------------------------------------------ conditioning
@@ -523,7 +529,7 @@ class WanDiTEngine:
         if hit is not None:
             return hit
         d, dev, nl = self.dim, self.device, len(self.blocks)
-        fd = self.model.freq_dim
+        fd = self.freq_dim
         te = sinusoidal_embedding_1d(fd, torch.tensor([tv], dtype=torch.float64)).to(torch.float32).to(dev)
         te2 = torch.empty(1, 2 * fd, device=dev, dtype=torch.bfloat16)
         th, t = (torch.empty(1, d, device=dev, dtype=torch.float32) for _ in range(2))
@@ -562,7 +568,7 @@ class WanDiTEngine:
         src = ctx_in.to(device=dev, dtype=torch.float32).contiguous()
         c2 = torch.empty(n_txt, 2 * td, device=dev, dtype=torch.bfloat16)
         self.k.split_f32_to_bf16x2(src, c2)
-        n_img = 257 if self.model.has_image_input else 0
+        n_img = 257 if self.has_image_input else 0
         emb = torch.empty(n_img + n_txt, d, device=dev, dtype=torch.bfloat16)
         hid = torch.empty(n_txt, d, device=dev, dtype=torch.float32)
         hid2 = torch.empty(n_txt, 2 * d, device=dev, dtype=torch.bfloat16)
@@ -619,7 +625,7 @@ class WanDiTEngine:
         """SVI-Talk: AudioProjModel (reference wan_video_dit.py:82-112) on the (first-frame, latter-frames) wav2vec window
         features, then every layer's audio K|V projection (models/attention.py:333-337) — all step-invariant, computed
         once per clip and branch.  audio_embed_tuple: ([1,1,5,12,768], [1,n,8,12,768])."""
-        if not getattr(self.model, "enable_multitalk", False):
+        if not self.enable_multitalk:
             raise RuntimeError("svi_b200: audio conditioning needs a WanModel built with enable_multitalk=True")
         dev, d = self.device, self.dim
         a0, a1 = audio_embed_tuple
@@ -794,7 +800,7 @@ class WanDiTEngine:
             raise RuntimeError(f"svi_b200: DiT forward expects x of shape [1,C,f,h,w], got {tuple(x.shape)}")
         xs = x[0].to(device=dev, dtype=torch.float32).contiguous()
         ys = None
-        if self.model.has_image_input:
+        if self.has_image_input:
             if y is None:
                 raise RuntimeError("has_image_input model needs y")
             ys = y[0].to(device=dev, dtype=torch.float32).contiguous()
@@ -897,7 +903,7 @@ class WanDiTEngine:
         # x = [add_condition +] patchify(x); with the fold its last pass also emits block 0's first operand + row statistics
         self._gemm_split(tok_l, self.w_patch, xr, bias=self.b_patch, residual=cond_l,
                          emit=None if fold is None else (h0, fold.v.g[0, 0], fold.stats[0, 0]))
-        if tea_cache is not None and tea_cache.check(self.model, xr, ts.t_mod):
+        if tea_cache is not None and tea_cache.check(None, xr, ts.t_mod):
             tea_cache.update(xr)                      # skipped step: tokens + residual of the last computed step
         else:
             row_sums = self._row_sums(Ll)
@@ -950,11 +956,17 @@ class WanModel(nn.Module):
         self._engine: Optional[WanDiTEngine] = None
         self._sig_params = None
         # unmerged LoRA adapters (plain attributes, not parameters or buffers: state_dict and the fingerprints ignore them)
-        self._lora_adapters = {}      # name -> ({(block, module): (A bf16 [r, in], B bf16 [out, r])}, default alpha)
-        self._lora_active = {}        # name -> alpha, in stacking order
-        self._lora_version = 0        # bumped when the active set or an active adapter's weights change
+        # adapters: name -> ({(block, module): (A bf16 [r, in], B bf16 [out, r])}, default alpha); active: name -> alpha,
+        # in stacking order; version: bumped when the active set or an active adapter's weights change.  One holder that
+        # the engine shares, so the engine needs no reference to the model.
+        self._lora_state = types.SimpleNamespace(adapters={}, active={}, version=0)
+        self._lora_adapters = self._lora_state.adapters
 
     # -- unmerged LoRA adapters ----------------------------------------------------------------
+    @property
+    def _lora_active(self):
+        return self._lora_state.active
+
     def add_lora_adapter(self, name, state_dict, alpha=1.0):
         """Register a LoRA (peft keys, as ModelManager.load_lora_v2 takes them) under `name` without merging it: it runs as
         a second K segment of the block GEMMs once set_lora_adapters activates it.  Targets: q, k, v, o of the self- and
@@ -962,8 +974,8 @@ class WanModel(nn.Module):
         The factors are kept in bf16 on the CPU; `alpha` is the scale set_lora_adapters uses when given names only."""
         from .lora import adapter_weights
         self._lora_adapters[name] = (adapter_weights(self, state_dict), float(alpha))
-        if name in self._lora_active:
-            self._lora_version += 1
+        if name in self._lora_state.active:
+            self._lora_state.version += 1
 
     def set_lora_adapters(self, adapters):
         """The active adapters: {name: alpha, ...} (stacked in this order, ranks concatenated, like several LoRA files
@@ -979,17 +991,18 @@ class WanModel(nn.Module):
         if unknown:
             raise ValueError(f"unknown LoRA adapter(s) {unknown}; loaded: {sorted(self._lora_adapters)}")
         new = {n: float(a) for n, a in adapters.items()}
-        if list(new) != list(self._lora_active):
-            self._lora_version += 1
-        self._lora_active = new
+        st = self._lora_state
+        if list(new) != list(st.active):
+            st.version += 1
+        st.active = new
 
     def delete_lora_adapter(self, name):
         """Forget an adapter (and deactivate it)."""
         if name not in self._lora_adapters:
             raise ValueError(f"unknown LoRA adapter {name!r}")
         del self._lora_adapters[name]
-        if name in self._lora_active:
-            self.set_lora_adapters({n: a for n, a in self._lora_active.items() if n != name})
+        if name in self._lora_state.active:
+            self.set_lora_adapters({n: a for n, a in self._lora_state.active.items() if n != name})
 
     # -- engine management -------------------------------------------------------------------
     def _param_signature(self):
