@@ -10,6 +10,8 @@ _LAZY = {
     "WanVideoPipeline": ("diffsynth.pipelines.wan_video", "WanVideoPipeline"),
     "WanUniAnimateVideoPipeline": ("diffsynth.pipelines.wan_video", "WanUniAnimateVideoPipeline"),
     "WanUniAnimateLongVideoPipeline": ("diffsynth.pipelines.wan_video", "WanUniAnimateLongVideoPipeline"),
+    "WanRepalceAnyoneVideoPipeline": ("diffsynth.pipelines.wan_video", "WanRepalceAnyoneVideoPipeline"),
+    "WanReplaceAnyoneVideoPipeline": ("diffsynth.pipelines.wan_video", "WanReplaceAnyoneVideoPipeline"),
     "SVIDanceVideoPipeline": ("diffsynth.pipelines.svi_video_dance", "SVIDanceVideoPipeline"),
     "SVITalkVideoPipeline": ("diffsynth.pipelines.svi_video_talk", "SVITalkVideoPipeline"),
     "save_video": ("diffsynth.data.video", "save_video"),

@@ -1,6 +1,6 @@
 """ctypes binding of the C-ABI kernel library ``libsvi_b200.so`` (declared in ``include/svi_b200.h``,
 ``include/svi_b200_lora.h``, ``include/svi_b200_rife.h``, ``include/svi_b200_esrgan.h``,
-``include/svi_b200_fastblend.h`` and ``include/svi_b200_unianimate.h``).
+``include/svi_b200_fastblend.h``, ``include/svi_b200_unianimate.h`` and ``include/svi_b200_replace.h``).
 
 This is the only door between the Python host code and the hand-written sm_90a kernels.  There is no
 fallback: if the shared library is missing or a call fails, a ``RuntimeError`` is raised.
@@ -223,6 +223,12 @@ UNIANIMATE_SIGNATURES = {
     "svi_window_normalize": (_i32, [_vp, _vp, _i32, _i32, _i64, _vp, _vp]),
 }
 
+# the same for include/svi_b200_replace.h
+REPLACE_SIGNATURES = {
+    "svi_replace_mask_stage": (_i32, [_vp, _vp, _i32, _i32, _i64, _vp, _vp, _i32, _vp]),
+}
+SEG_U8, SEG_F32 = 0, 1
+
 _lib = None
 
 
@@ -241,7 +247,7 @@ def load():
             f"`python -c 'import __graft_entry__ as g; g.build()'` (or `make`) — there is no CPU fallback.")
     lib = ctypes.CDLL(_LIB_PATH)
     for name, (res, args) in (SIGNATURES | LORA_SIGNATURES | RIFE_SIGNATURES | ESRGAN_SIGNATURES |
-                        FASTBLEND_SIGNATURES | UNIANIMATE_SIGNATURES).items():
+                        FASTBLEND_SIGNATURES | UNIANIMATE_SIGNATURES | REPLACE_SIGNATURES).items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing: fail loudly
         fn.restype = res
         fn.argtypes = args
@@ -1120,3 +1126,28 @@ def window_normalize(sum_, count, out):
     _check(load().svi_window_normalize(_ptr(sum_, torch.float32, "sum"), _ptr(count, torch.int32, "count"), C, F, hw,
                                        _ptr(out, torch.float32, "out"), _stream()), "svi_window_normalize")
     return out
+
+
+# --------------------------------------------------------------------------------------------- Replace-Anyone (include/svi_b200_replace.h)
+def replace_mask_stage(video, seg, masked, ring):
+    """video f32 [3, T, H, W], seg uint8 or f32 [T, H, W] (contiguous) -> masked f32 [3, T, H, W] (or None) =
+    video * keep, and ring bf16 [T, H, W, ldr] channels 0..3 = (masked, keep), keep = !(seg / 255 > 0)
+    (svi_replace_mask_stage)."""
+    if video.dim() != 4 or video.shape[0] != 3 or not video.is_contiguous():
+        raise RuntimeError(f"svi_b200.replace_mask_stage: video must be a contiguous [3, T, H, W] tensor, got {tuple(video.shape)}")
+    _, T, H, W = video.shape
+    if tuple(seg.shape) != (T, H, W) or not seg.is_contiguous():
+        raise RuntimeError(f"svi_b200.replace_mask_stage: seg must be a contiguous [T, H, W] = {(T, H, W)} tensor, "
+                           f"got {tuple(seg.shape)}")
+    seg_type = {torch.uint8: SEG_U8, torch.float32: SEG_F32}.get(seg.dtype)
+    if seg_type is None:
+        raise RuntimeError(f"svi_b200.replace_mask_stage: seg must be uint8 or float32, got {seg.dtype}")
+    if masked is not None and (masked.shape != video.shape or not masked.is_contiguous()):
+        raise RuntimeError("svi_b200.replace_mask_stage: masked must be contiguous and shaped like video")
+    if ring.dim() != 4 or tuple(ring.shape[:3]) != (T, H, W) or not ring.is_contiguous():
+        raise RuntimeError(f"svi_b200.replace_mask_stage: ring must be a contiguous [T, H, W, ldr] = {(T, H, W)} + (ldr,) "
+                           f"tensor, got {tuple(ring.shape)}")
+    _check(load().svi_replace_mask_stage(_ptr(video, torch.float32, "video"), _ptr(seg, name="seg"), seg_type, T, H * W,
+                                         _ptr(masked, torch.float32, "masked"), _ptr(ring, torch.bfloat16, "ring"),
+                                         ring.shape[3], _stream()), "svi_replace_mask_stage")
+    return masked, ring

@@ -16,6 +16,12 @@ UniAnimate-DiT adds a second, 2-D stem on a single reference-pose image (``rando
 ``pipelines/wan_video.py:543-558``): six ``nn.Conv2d`` 3x3 / padding 1 (3 -> 16 -> 16 -> 16 -> 16 -> 16 -> 20 channels,
 strides 1, 1, 1, 2, 2, 2, SiLU after all but the last).  ``RandomRefEmbeddingEngine`` runs it on the same conv launch as
 the 3-D stem with one frame and kt = 1.
+
+The Replace-Anyone model of UniAnimate-DiT adds two more 3-D stems (reference ``pipelines/wan_video.py:1353-1369``), both
+3x3x3 / padding 1 with SiLU between the convs: ``learn_in_embedding`` (4 -> 16 -> 16 -> 16 -> 16 channels, strides 1,
+(1, 2, 2), 2, 2) on the masked video and its keep mask, and ``inpaint_embedding`` (16 -> 16 -> 16 -> 16, stride 1) on the
+VAE latents of the masked video.  ``LearnInEmbeddingEngine`` and ``InpaintEmbeddingEngine`` run them on the pose stem's
+layer loop (``_StemEngine._layers``).
 """
 import torch
 import torch.nn as nn
@@ -112,6 +118,37 @@ class _StemEngine:
             self.launches += 1
         return out
 
+    def _layers(self, full, down, t_strides, stage, frames, H, W):
+        """The layer sequence of the 3-D stems: full-resolution convs (stride 1), then convs with spatial stride 2 and
+        temporal strides `t_strides`, all 3x3x3 with padding 1 and SiLU between them.  `stage(ring)` writes the first
+        conv's input into a ring of max(frames) + 1 frames; `frames` maps that conv's input frames to ring slots, so a
+        repeated slot repeats a frame without a copy.  The later full-resolution convs restage frame t into slot t, which
+        needs a ring of at least len(frames) frames.  Returns the last conv's f32 output [T, H', W', c_out]."""
+        dev = self.device
+        # ---- full-resolution convs: one ring holds the input frames (+ the zero slot) and is re-staged layer by layer
+        ring = _Ring(max(frames) + 1, H, W, full[0].c_in, dev, history=0)
+        stage(ring)
+        T = len(frames)
+        x = self._conv(full[0], ring, frames, T, 1, H, W)
+        for cv in full[1:]:
+            for t in range(T):
+                xt = x[t]                                                                     # [H, W, c] f32
+                nv.vae_norm_act(xt, H * W, xt.shape[-1], xt.stride(1), None, True, ring.buf[t], ring.C)   # SiLU -> bf16
+                self.launches += 1
+            x = self._conv(cv, ring, list(range(T)), T, 1, H, W)
+        del ring
+        # ---- strided convs: SiLU + space-to-depth staging, 2x2 spatial taps, temporal stride through the slot table
+        for cv, ts in zip(down, t_strides):
+            Tn, Hn, Wn, Cn = x.shape
+            ring = _Ring(Tn, Hn // 2, Wn // 2, 4 * Cn, dev, history=0)
+            for t in range(Tn):
+                nv.vae_space_to_depth_act(x[t], Hn, Wn, Cn, nv.ACT_SILU, ring.buf[t])
+                self.launches += 1
+            T_out = (Tn + 2 - 3) // ts + 1
+            x = self._conv(cv, ring, list(range(Tn)), T_out, ts, Hn // 2, Wn // 2)
+            del ring
+        return x
+
 
 class DWPoseEmbeddingEngine(_StemEngine):
     def __init__(self, seq: nn.Sequential, device):
@@ -127,32 +164,14 @@ class DWPoseEmbeddingEngine(_StemEngine):
         if C != 3 or H % 16 or W % 16:
             raise RuntimeError(f"svi_b200: pose video must be [3, T, H, W] with H, W multiples of 16, got {tuple(pose.shape)}")
         pose = pose.to(device=dev, dtype=torch.float32).contiguous()
-        # ---- full-resolution convs: one ring holds all T frames (+ the zero slot) and is re-staged layer by layer
-        ring = _Ring(T, H, W, self.full[0].c_in, dev, history=0)
-        frames = list(range(T))
-        xin = torch.empty(H, W, 8, device=dev, dtype=torch.float32)
-        for t in range(T):
-            nv.vae_from_planar(pose[:, t], 3, H * W, None, None, xin, 8, False, ldc=T * H * W)
-            nv.vae_norm_act(xin, H * W, 8, 8, None, False, ring.buf[t], ring.C)
-            self.launches += 2
-        x = self._conv(self.full[0], ring, frames, T, 1, H, W)
-        for cv in self.full[1:]:
+
+        def stage(ring):
+            xin = torch.empty(H, W, 8, device=dev, dtype=torch.float32)
             for t in range(T):
-                xt = x[t]                                                                     # [H, W, c] f32
-                nv.vae_norm_act(xt, H * W, xt.shape[-1], xt.stride(1), None, True, ring.buf[t], ring.C)   # SiLU -> bf16
-                self.launches += 1
-            x = self._conv(cv, ring, frames, T, 1, H, W)
-        del ring
-        # ---- strided convs: SiLU + space-to-depth staging, 2x2 spatial taps, temporal stride through the slot table
-        for cv, ts in zip(self.down, self.t_stride):
-            Tn, Hn, Wn, Cn = x.shape
-            ring = _Ring(Tn, Hn // 2, Wn // 2, 4 * Cn, dev, history=0)
-            for t in range(Tn):
-                nv.vae_space_to_depth_act(x[t], Hn, Wn, Cn, nv.ACT_SILU, ring.buf[t])
-                self.launches += 1
-            T_out = (Tn + 2 - 3) // ts + 1
-            x = self._conv(cv, ring, list(range(Tn)), T_out, ts, Hn // 2, Wn // 2)
-            del ring
+                nv.vae_from_planar(pose[:, t], 3, H * W, None, None, xin, 8, False, ldc=T * H * W)
+                nv.vae_norm_act(xin, H * W, 8, 8, None, False, ring.buf[t], ring.C)
+                self.launches += 2
+        x = self._layers(self.full, self.down, self.t_stride, stage, list(range(T)), H, W)
         # ---- projection: SiLU, (1,2,2)/(1,2,2) conv = space-to-depth + GEMM to the DiT width
         Tn, Hn, Wn, Cn = x.shape
         a = torch.zeros(Tn, Hn // 2, Wn // 2, self.kproj, device=dev, dtype=torch.bfloat16)
@@ -227,4 +246,86 @@ class RandomRefEmbeddingEngine(_StemEngine):
             nv.vae_space_to_depth_act(x[0], Hn, Wn, Cn, nv.ACT_SILU, ring.buf[0])
             self.launches += 1
             x = self._conv(cv, ring, [0], 1, 1, Hn // 2, Wn // 2)
+        return x[..., :self.out_channels].permute(3, 0, 1, 2).unsqueeze(0).contiguous()
+
+
+def make_learn_in_embedding(concat_dim=4):
+    """The masked-video stem of UniAnimate-DiT Replace-Anyone (reference wan_video.py:1353-1361), keys `0.weight` ...
+    `6.bias`."""
+    c = concat_dim * 4
+    return nn.Sequential(
+        nn.Conv3d(4, c, (3, 3, 3), stride=(1, 1, 1), padding=(1, 1, 1)), nn.SiLU(),
+        nn.Conv3d(c, c, (3, 3, 3), stride=(1, 2, 2), padding=(1, 1, 1)), nn.SiLU(),
+        nn.Conv3d(c, c, 3, stride=(2, 2, 2), padding=1), nn.SiLU(),
+        nn.Conv3d(c, 16, 3, stride=2, padding=1))
+
+
+def make_inpaint_embedding(concat_dim=4):
+    """The masked-latent stem of UniAnimate-DiT Replace-Anyone (reference wan_video.py:1363-1369), keys `0.weight` ...
+    `4.bias`."""
+    c = concat_dim * 4
+    return nn.Sequential(
+        nn.Conv3d(16, c, (3, 3, 3), stride=(1, 1, 1), padding=(1, 1, 1)), nn.SiLU(),
+        nn.Conv3d(c, c, 3, stride=(1, 1, 1), padding=1), nn.SiLU(),
+        nn.Conv3d(c, 16, 3, stride=1, padding=1))
+
+
+def _convs3d(seq, strides, what):
+    convs = [m for m in seq if isinstance(m, nn.Conv3d)]
+    if [tuple(m.stride) for m in convs] != strides or any(tuple(m.kernel_size) != (3, 3, 3) for m in convs):
+        raise RuntimeError(f"{what} must be the {len(strides)}-conv stem of wan_video.py:1353-1369")
+    return convs
+
+
+class LearnInEmbeddingEngine(_StemEngine):
+    """The masked-video stem.  Its first ring is written by svi_replace_mask_stage straight from the video and the
+    segmentation; the three leading repeats of frame 0 are slot-table entries, not copies."""
+
+    def __init__(self, seq: nn.Sequential, device):
+        super().__init__(device, "the learn-in stem")
+        convs = _convs3d(seq, [(1, 1, 1), (1, 2, 2), (2, 2, 2), (2, 2, 2)], "learn_in_embedding")
+        self.full = [_Conv(convs[0].weight, convs[0].bias, self.device)]
+        self.down = [_Conv(m.weight, m.bias, self.device, s2d="before") for m in convs[1:]]
+        self.t_stride = [m.stride[0] for m in convs[1:]]
+        self.out_channels = convs[-1].out_channels
+
+    def forward(self, video, seg, masked=None):
+        """video f32 [3, T, H, W], seg uint8 or f32 [T, H, W] (on the device, contiguous) -> f32
+        [1, 16, f, H/8, W/8] of cat([m[:, :1] x3, m]) with m = cat([video * keep, keep]), keep = !(seg / 255 > 0).
+        `masked` (f32 [3, T, H, W] or None) receives video * keep, the VAE encoder's input."""
+        C, T, H, W = video.shape
+        if C != 3 or H % 8 or W % 8:
+            raise RuntimeError(f"svi_b200: the learn-in stem needs a [3, T, H, W] video with H, W multiples of 8, "
+                               f"got {tuple(video.shape)}")
+
+        def stage(ring):
+            nv.replace_mask_stage(video, seg, masked, ring.buf[:T])
+            self.launches += 1
+        x = self._layers(self.full, self.down, self.t_stride, stage, [0, 0, 0] + list(range(T)), H, W)
+        return x[..., :self.out_channels].permute(3, 0, 1, 2).unsqueeze(0).contiguous()
+
+
+class InpaintEmbeddingEngine(_StemEngine):
+    """The masked-latent stem: the f32 planar latents staged to the bf16 ring by svi_vae_from_planar, three stride-1
+    convs."""
+
+    def __init__(self, seq: nn.Sequential, device):
+        super().__init__(device, "the inpaint stem")
+        convs = _convs3d(seq, [(1, 1, 1)] * 3, "inpaint_embedding")
+        self.full = [_Conv(m.weight, m.bias, self.device) for m in convs]
+        self.in_channels, self.out_channels = convs[0].in_channels, convs[-1].out_channels
+
+    def forward(self, latents):
+        """latents f32 [1, C, f, h, w] -> f32 [1, out_channels, f, h, w]."""
+        dev = self.device
+        lat = latents.to(device=dev, dtype=torch.float32).contiguous()
+        _, C, F, h, w = lat.shape
+        if C != self.in_channels:
+            raise RuntimeError(f"svi_b200: the inpaint stem needs {self.in_channels}-channel latents, got {tuple(lat.shape)}")
+
+        def stage(ring):
+            for t in range(F):
+                nv.vae_from_planar(lat[0, :, t], C, h * w, None, None, ring.buf[t], ring.C, True, ldc=F * h * w)
+                self.launches += 1
+        x = self._layers(self.full, [], [], stage, list(range(F)), h, w)
         return x[..., :self.out_channels].permute(3, 0, 1, 2).unsqueeze(0).contiguous()

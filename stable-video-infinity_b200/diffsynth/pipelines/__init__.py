@@ -1,2 +1,3 @@
 from .svi_video import SVIVideoPipeline
-from .wan_video import WanUniAnimateLongVideoPipeline, WanUniAnimateVideoPipeline, WanVideoPipeline
+from .wan_video import (WanRepalceAnyoneVideoPipeline, WanReplaceAnyoneVideoPipeline, WanUniAnimateLongVideoPipeline,
+                        WanUniAnimateVideoPipeline, WanVideoPipeline)

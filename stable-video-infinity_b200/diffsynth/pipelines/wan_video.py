@@ -10,15 +10,18 @@
   overlapping windows of ``context_size`` latent frames and averages them per frame (``svi_window_accumulate`` /
   ``svi_window_normalize``).
 
-``WanRepalceAnyoneVideoPipeline`` (:1207-1583) is not provided: its ``__call__`` reads an undefined ``batch``.
+* ``WanRepalceAnyoneVideoPipeline`` (:1207-1584, also exported as ``WanReplaceAnyoneVideoPipeline``), UniAnimate-DiT
+  Replace-Anyone: re-animates the person masked out of ``batch["video"]`` by ``batch["segmentation_data"]`` (the
+  ``batch`` keyword of its ``__call__``, :1488) with the identity of ``input_image`` and the pose of ``dwpose_data``.
 """
 import numpy as np
 import torch
 from tqdm import tqdm
 
 from .. import _native as nv
-from ..models.dwpose_embedding import (DWPoseEmbeddingEngine, RandomRefEmbeddingEngine, make_dwpose_embedding,
-                                       make_randomref_embedding_pose, pose_condition)
+from ..models.dwpose_embedding import (DWPoseEmbeddingEngine, InpaintEmbeddingEngine, LearnInEmbeddingEngine,
+                                       RandomRefEmbeddingEngine, make_dwpose_embedding, make_inpaint_embedding,
+                                       make_learn_in_embedding, make_randomref_embedding_pose, pose_condition)
 from .svi_video import SVIVideoPipeline, TeaCache, model_fn_wan_video  # noqa: F401  (re-exported like the reference)
 
 
@@ -81,6 +84,11 @@ class WanVideoPipeline(SVIVideoPipeline):
         return self.tensor2video(frames[0])
 
 
+def _stem_keys(state_dict_new_module, tag):
+    """The keys of one extra module with everything up to `tag` removed ('pipe.dwpose_embedding.0.weight' -> '0.weight')."""
+    return {k.split(tag)[1]: v for k, v in state_dict_new_module.items() if tag in k}
+
+
 class WanUniAnimateVideoPipeline(WanVideoPipeline):
     """UniAnimate-DiT on one clip (reference wan_video.py:411-757)."""
 
@@ -99,14 +107,12 @@ class WanUniAnimateVideoPipeline(WanVideoPipeline):
         """Build both stems from the extra-module keys load_lora_v2 keeps (`...dwpose_embedding.N.*`,
         `...randomref_embedding_pose.N.*`; strict, like the reference :559-570).  A stem whose keys are absent stays
         None.  The pose stem's output width is the checkpoint's (the reference hard-codes 5120, :541)."""
-        def part(tag):
-            return {k.split(tag)[1]: v for k, v in state_dict_new_module.items() if tag in k}
-        sd = part("dwpose_embedding.")
+        sd = _stem_keys(state_dict_new_module, "dwpose_embedding.")
         if sd:
             self.dwpose_embedding = make_dwpose_embedding(dim=sd["12.weight"].shape[0])
             self.dwpose_embedding.load_state_dict(sd, strict=True)
             self._pose_engine = None
-        sd = part("randomref_embedding_pose.")
+        sd = _stem_keys(state_dict_new_module, "randomref_embedding_pose.")
         if sd:
             self.randomref_embedding_pose = make_randomref_embedding_pose(randomref_dim=sd["10.weight"].shape[0])
             self.randomref_embedding_pose.load_state_dict(sd, strict=True)
@@ -325,3 +331,146 @@ class WanUniAnimateLongVideoPipeline(WanUniAnimateVideoPipeline):
                 nv.window_accumulate(win, 0 if k == 0 else 2, acc, s)
             nv.window_normalize(acc, count, lat)
         return lat
+
+
+class WanRepalceAnyoneVideoPipeline(WanUniAnimateVideoPipeline):
+    """UniAnimate-DiT Replace-Anyone (reference wan_video.py:1207-1584; the class name keeps the reference's spelling,
+    ``WanReplaceAnyoneVideoPipeline`` is the same class).
+
+    ``batch = {"video": [3, num_frames, height, width] float in [-1, 1], "segmentation_data": [1, num_frames, height,
+    width] uint8 or float, > 0 on the person to replace}``.  Once per call the video with the person cut out,
+    ``video * keep`` with ``keep = !(segmentation_data / 255 > 0)``, goes through the VAE encoder and the inpaint stem, and
+    together with ``keep`` through the learn-in stem (svi_replace_mask_stage stages both); the sum of the two results,
+    each rounded to bf16 as the reference does, is the offset of the conditional branch.  Every step the conditional
+    forward sees latents + offset and the pose tokens, the unconditional forward the plain latents and no pose tokens.
+    That asymmetry is the reference's (:1566, :1569).  Latents, the offset and latents + offset are f32; the reference
+    keeps them in the pipeline dtype."""
+
+    def __init__(self, device="cuda", torch_dtype=torch.float16, tokenizer_path=None):
+        super().__init__(device=device, torch_dtype=torch_dtype, tokenizer_path=tokenizer_path)
+        self.learn_in_embedding = None
+        self.inpaint_embedding = None
+        self._learn_in_engine = None
+        self._inpaint_engine = None
+
+    def fetch_models(self, model_manager):
+        super().fetch_models(model_manager)
+        self.load_replace_stems(model_manager.state_dict_new_module)
+
+    def load_replace_stems(self, state_dict_new_module):
+        """Build the learn-in and inpaint stems from the extra-module keys load_lora_v2 keeps (`...learn_in_embedding.N.*`,
+        `...inpaint_embedding.N.*`; strict, like the reference :1384-1395).  A stem whose keys are absent stays None."""
+        sd = _stem_keys(state_dict_new_module, "learn_in_embedding.")
+        if sd:
+            self.learn_in_embedding = make_learn_in_embedding()
+            self.learn_in_embedding.load_state_dict(sd, strict=True)
+            self._learn_in_engine = None
+        sd = _stem_keys(state_dict_new_module, "inpaint_embedding.")
+        if sd:
+            self.inpaint_embedding = make_inpaint_embedding()
+            self.inpaint_embedding.load_state_dict(sd, strict=True)
+            self._inpaint_engine = None
+
+    @staticmethod
+    def from_model_manager(model_manager, torch_dtype=None, device=None):
+        device = model_manager.device if device is None else device
+        torch_dtype = model_manager.torch_dtype if torch_dtype is None else torch_dtype
+        pipe = WanRepalceAnyoneVideoPipeline(device=device, torch_dtype=torch_dtype)
+        pipe.fetch_models(model_manager)
+        return pipe
+
+    @staticmethod
+    def _check_batch(batch, num_frames, height, width):
+        if batch is None or "video" not in batch or "segmentation_data" not in batch:
+            raise ValueError('Replace-Anyone needs batch={"video": [3, num_frames, height, width], '
+                             '"segmentation_data": [1, num_frames, height, width]}')
+        video, seg = batch["video"], batch["segmentation_data"]
+        if not torch.is_tensor(video) or tuple(video.shape) != (3, num_frames, height, width):
+            raise ValueError(f'batch["video"] must be a tensor [3, num_frames, height, width] = '
+                             f'{(3, num_frames, height, width)} (num_frames after rounding to 4k+1, height and width '
+                             f'after rounding to multiples of 16), got {tuple(getattr(video, "shape", ()))}')
+        if not torch.is_tensor(seg) or tuple(seg.shape) != (1, num_frames, height, width):
+            raise ValueError(f'batch["segmentation_data"] must be a tensor [1, num_frames, height, width] = '
+                             f'{(1, num_frames, height, width)}, got {tuple(getattr(seg, "shape", ()))}')
+        return video, seg
+
+    def encode_masked_video(self, video, segmentation_data, tiler_kwargs):
+        """video [3, T, H, W], segmentation_data [1, T, H, W] -> the conditional branch's offset, f32 [1, 16, f, h, w]:
+        bf16(learn_in_embedding(...)) + bf16(inpaint_embedding(VAE(video * keep))) (reference :1545-1555)."""
+        if self.learn_in_embedding is None or self.inpaint_embedding is None:
+            raise RuntimeError("svi_b200: no learn-in or inpaint stem loaded (learn_in_embedding.* and inpaint_embedding.* "
+                               "keys of the UniAnimate-DiT Replace-Anyone checkpoint)")
+        if self._learn_in_engine is None:
+            self._learn_in_engine = LearnInEmbeddingEngine(self.learn_in_embedding, self.device)
+        if self._inpaint_engine is None:
+            self._inpaint_engine = InpaintEmbeddingEngine(self.inpaint_embedding, self.device)
+        dev = self.device
+        video = video.to(device=dev, dtype=torch.float32).contiguous()
+        seg = segmentation_data[0].to(dev)
+        if seg.dtype not in (torch.uint8, torch.float32):
+            seg = seg.to(torch.float32)
+        masked = torch.empty_like(video)
+        learn_in = self._learn_in_engine.forward(video, seg.contiguous(), masked)
+        lat_masked = self.encode_video(masked.unsqueeze(0), **tiler_kwargs).to(torch.float32)
+        inpaint = self._inpaint_engine.forward(lat_masked)
+        return nv.axpby(learn_in.to(torch.bfloat16).to(torch.float32), 1.0,
+                        inpaint.to(torch.bfloat16).to(torch.float32), 1.0, learn_in)
+
+    @torch.no_grad()
+    def __call__(self, prompt, negative_prompt="", input_image=None, input_video=None, denoising_strength=1.0, seed=None,
+                 rand_device="cpu", height=480, width=832, num_frames=81, cfg_scale=5.0, num_inference_steps=50,
+                 sigma_shift=5.0, tiled=True, tile_size=(30, 52), tile_stride=(15, 26), tea_cache_l1_thresh=None,
+                 tea_cache_model_id="", progress_bar_cmd=tqdm, progress_bar_st=None, dwpose_data=None,
+                 random_ref_dwpose=None, batch=None):
+        height, width = self.check_resize_height_width(height, width)
+        if num_frames % 4 != 1:
+            num_frames = (num_frames + 2) // 4 * 4 + 1
+            print(f"Only `num_frames % 4 != 1` is acceptable. We round it up to {num_frames}.")
+        self._check_inputs(input_image, dwpose_data, random_ref_dwpose, num_frames, height, width)
+        video, seg = self._check_batch(batch, num_frames, height, width)
+        tiler_kwargs = {"tiled": tiled, "tile_size": tile_size, "tile_stride": tile_stride}
+        self.scheduler.set_timesteps(num_inference_steps, denoising_strength=denoising_strength, shift=sigma_shift)
+        latents = self._initial_latents(num_frames, height, width, seed, rand_device, input_video, tiler_kwargs)
+        pos = self.encode_prompt(prompt, positive=True)
+        neg = self.encode_prompt(negative_prompt, positive=False) if cfg_scale != 1.0 else None
+        image_emb = self.encode_image(input_image, num_frames, height, width)
+        condition = self.encode_pose(dwpose_data)
+        y = image_emb["y"] + self.encode_ref_pose(random_ref_dwpose)
+        offset = self.encode_masked_video(video, seg, tiler_kwargs)
+        bar = (lambda r: progress_bar_cmd(r)) if progress_bar_cmd is not None else (lambda r: r)
+        mk = lambda: (TeaCache(num_inference_steps, rel_l1_thresh=tea_cache_l1_thresh, model_id=tea_cache_model_id)
+                      if tea_cache_l1_thresh is not None else None)
+        latents = self.denoise_replace(latents, offset, pos["context"], None if neg is None else neg["context"],
+                                       image_emb["clip_feature"], y, cfg_scale, condition, (mk(), mk()), bar)
+        frames = self.decode_video(latents, **tiler_kwargs)
+        return self.tensor2video(frames[0])
+
+    def denoise_replace(self, latents, offset, context_posi, context_nega, clip_feature, y, cfg_scale, condition,
+                        tea=(None, None), progress_bar_cmd=lambda x: x):
+        """The loop of :1562-1575.  latents f32 [1, 16, f, h, w]; offset f32 of the same shape.  Per step: x_c = latents +
+        offset (svi_axpby), the conditional forward on x_c with the pose tokens, the unconditional forward on the
+        latents without them, one fused CFG + Euler step on the latents.  Returns the denoised f32 latents."""
+        eng = self.dit.engine(self.device)
+        dev = self.device
+        lat = latents.to(device=dev, dtype=torch.float32).contiguous()
+        offset = offset.to(device=dev, dtype=torch.float32).contiguous()
+        y = y.to(device=dev, dtype=torch.float32).contiguous()
+        cp = eng.context_state(context_posi, clip_feature)
+        cn = eng.context_state(context_nega, clip_feature) if cfg_scale != 1.0 else None
+        x_c = torch.empty_like(lat)
+        v_c = torch.empty_like(lat)
+        v_u = torch.empty_like(lat) if cn is not None else None
+        sig = self.scheduler.sigmas
+        ts = self.scheduler.timesteps
+        n = len(ts)
+        for i in progress_bar_cmd(range(n)):
+            nxt = float(sig[i + 1]) if i + 1 < n else 0.0
+            eng.k.axpby(lat, 1.0, offset, 1.0, x_c)
+            eng.forward(x_c, float(ts[i]), cp, y=y, out=v_c, tea_cache=tea[0], add_condition=condition)
+            if cn is not None:
+                eng.forward(lat, float(ts[i]), cn, y=y, out=v_u, tea_cache=tea[1])
+            eng.k.cfg_euler_step(lat, v_c, v_u, cfg_scale, float(sig[i]), nxt)
+        return lat
+
+
+WanReplaceAnyoneVideoPipeline = WanRepalceAnyoneVideoPipeline
