@@ -910,7 +910,12 @@ def rife_conv2d(x, w, kh, kw, pad, C_out, phase_cols, bias, tile_w, prelu=None, 
             raise RuntimeError("svi_b200.rife_conv2d: out_bf16 must be [N, ., ., bf_ld]")
         d.out_bf16, d.bf_img_stride, d.bf_ld = _contig(out_bf16, torch.bfloat16, "out_bf16"), out_bf16[0].numel(), out_bf16.shape[3]
         d.bf_s2d = int(bool(bf_s2d))
-    _check(load().svi_rife_conv2d(ctypes.byref(d), _stream()), "svi_rife_conv2d")
+    rife_conv2d_desc(d)
+
+
+def rife_conv2d_desc(desc):
+    """Launch svi_rife_conv2d with a filled RifeConvDesc (pointers as ints)."""
+    _check(load().svi_rife_conv2d(ctypes.byref(desc), _stream()), "svi_rife_conv2d")
 
 
 def rife_update_warp(heads, src_scale, flow_mul, img0, img1, state, first, merged=None, clip=False, rgb=None):
@@ -993,7 +998,12 @@ def esrgan_conv2d(x, w, C_out, bias, tile_w, slope=0.0, residual=None, res_scale
         if tuple(out_u8.shape) != (N, H, W, 3):
             raise RuntimeError("svi_b200.esrgan_conv2d: out_u8 must be [N, H, W, 3]")
         d.out_u8 = _contig(out_u8, torch.uint8, "out_u8")
-    _check(load().svi_esrgan_conv2d(ctypes.byref(d), _stream()), "svi_esrgan_conv2d")
+    esrgan_conv2d_desc(d)
+
+
+def esrgan_conv2d_desc(desc):
+    """Launch svi_esrgan_conv2d with a filled EsrganConvDesc (pointers as ints)."""
+    _check(load().svi_esrgan_conv2d(ctypes.byref(desc), _stream()), "svi_esrgan_conv2d")
 
 
 # --------------------------------------------------------------------------------------------- FastBlend (include/svi_b200_fastblend.h)
