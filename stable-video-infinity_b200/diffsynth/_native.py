@@ -1,6 +1,7 @@
 """ctypes binding of the C-ABI kernel library ``libsvi_b200.so`` (declared in ``include/svi_b200.h``,
 ``include/svi_b200_lora.h``, ``include/svi_b200_rife.h``, ``include/svi_b200_esrgan.h``,
-``include/svi_b200_fastblend.h``, ``include/svi_b200_unianimate.h`` and ``include/svi_b200_replace.h``).
+``include/svi_b200_fastblend.h``, ``include/svi_b200_unianimate.h``, ``include/svi_b200_replace.h`` and
+``include/svi_b200_quality.h``).
 
 This is the only door between the Python host code and the hand-written sm_90a kernels.  There is no
 fallback: if the shared library is missing or a call fails, a ``RuntimeError`` is raised.
@@ -229,6 +230,18 @@ REPLACE_SIGNATURES = {
 }
 SEG_U8, SEG_F32 = 0, 1
 
+# the same for include/svi_b200_quality.h
+QUALITY_SIGNATURES = {
+    "svi_quality_attn": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _f32, _i32, _vp]),
+    "svi_quality_stage_pixels": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _i32, _vp]),
+    "svi_quality_embed_ln": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _f32, _vp, _vp, _vp, _vp]),
+    "svi_quality_quick_gelu": (_i32, [_vp, _i64, _i32, _i32, _vp, _i64, _vp]),
+    "svi_quality_pool": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _i32, _i64, _vp, _vp]),
+    "svi_quality_score": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _f32, _vp, _vp, _vp]),
+}
+QUALITY_MAX_L = 320
+POOL_FIRST, POOL_ARGMAX, POOL_EOS = 0, 1, 2
+
 _lib = None
 
 
@@ -247,7 +260,7 @@ def load():
             f"`python -c 'import __graft_entry__ as g; g.build()'` (or `make`) — there is no CPU fallback.")
     lib = ctypes.CDLL(_LIB_PATH)
     for name, (res, args) in (SIGNATURES | LORA_SIGNATURES | RIFE_SIGNATURES | ESRGAN_SIGNATURES |
-                        FASTBLEND_SIGNATURES | UNIANIMATE_SIGNATURES | REPLACE_SIGNATURES).items():
+                        FASTBLEND_SIGNATURES | UNIANIMATE_SIGNATURES | REPLACE_SIGNATURES | QUALITY_SIGNATURES).items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing: fail loudly
         fn.restype = res
         fn.argtypes = args
@@ -1161,3 +1174,89 @@ def replace_mask_stage(video, seg, masked, ring):
                                          _ptr(masked, torch.float32, "masked"), _ptr(ring, torch.bfloat16, "ring"),
                                          ring.shape[3], _stream()), "svi_replace_mask_stage")
     return masked, ring
+
+
+# --------------------------------------------------------------------------------------------- quality scoring (include/svi_b200_quality.h)
+def quality_attn(q, k, v, out, batch, num_heads, head_dim, scale, causal=False):
+    """softmax(q k^T * scale [+ causal mask]) v for `batch` sequences of L = rows / batch tokens (svi_quality_attn); q, k,
+    v, out bf16 [batch * L, >= num_heads * head_dim] row-major views (column slices of the fused qkv output)."""
+    ldq, ldk, ldv, ldo = (_rowmajor(t, n) for t, n in ((q, "q"), (k, "k"), (v, "v"), (out, "out")))
+    rows = q.shape[0]
+    if batch < 1 or rows % batch or any(t.shape[0] != rows for t in (k, v, out)):
+        raise RuntimeError(f"svi_b200.quality_attn: q, k, v, out must have the same rows, a multiple of batch = {batch}")
+    _check(load().svi_quality_attn(_ptr(q, torch.bfloat16, "q"), ldq, _ptr(k, torch.bfloat16, "k"), ldk,
+                                   _ptr(v, torch.bfloat16, "v"), ldv, _ptr(out, torch.bfloat16, "out"), ldo, int(batch),
+                                   rows // batch, int(num_heads), int(head_dim), float(scale), int(bool(causal)), _stream()),
+           "svi_quality_attn")
+    return out
+
+
+def quality_stage_pixels(px, mean_std, out, patch):
+    """px f32 [B, 3, S, S] -> out bf16 [B * (S/patch)^2, kpad] = (px - mean) / std in patch rows (svi_quality_stage_pixels);
+    mean_std f32 [6] on the device."""
+    if px.dim() != 4 or px.shape[1] != 3 or px.shape[2] != px.shape[3] or not px.is_contiguous():
+        raise RuntimeError(f"svi_b200.quality_stage_pixels: px must be a contiguous [B, 3, S, S] tensor, got {tuple(px.shape)}")
+    B, _, S, _ = px.shape
+    if not out.is_contiguous() or out.dim() != 2 or out.shape[0] != B * (S // patch) ** 2:
+        raise RuntimeError("svi_b200.quality_stage_pixels: out must be a contiguous [B * (S/patch)^2, kpad] tensor")
+    if mean_std.numel() != 6 or not mean_std.is_contiguous():
+        raise RuntimeError("svi_b200.quality_stage_pixels: mean_std must hold 6 floats")
+    _check(load().svi_quality_stage_pixels(_ptr(px, torch.float32, "px"), B, S, int(patch),
+                                           _ptr(mean_std, torch.float32, "mean_std"), _ptr(out, torch.bfloat16, "out"),
+                                           out.shape[1], _stream()), "svi_quality_stage_pixels")
+    return out
+
+
+def quality_embed_ln(patch, cls, pos, gamma, beta, eps, out):
+    """out f32 [B*(1+np), D] = LayerNorm([cls; patch rows of image b] + pos) per image (svi_quality_embed_ln)."""
+    np_, D = pos.shape[0] - 1, pos.shape[1]
+    if patch.dim() != 2 or patch.shape[1] != D or patch.shape[0] % np_ or not patch.is_contiguous():
+        raise RuntimeError("svi_b200.quality_embed_ln: patch must be a contiguous [B * np, D] tensor")
+    B = patch.shape[0] // np_
+    if tuple(out.shape) != (B * (np_ + 1), D) or not out.is_contiguous() or not pos.is_contiguous():
+        raise RuntimeError("svi_b200.quality_embed_ln: out must be a contiguous [B * (np + 1), D] tensor")
+    if cls.numel() != D or gamma.numel() != D or beta.numel() != D:
+        raise RuntimeError("svi_b200.quality_embed_ln: cls, gamma and beta must hold D floats")
+    _check(load().svi_quality_embed_ln(_ptr(patch, torch.float32, "patch"), _ptr(cls, torch.float32, "cls"),
+                                       _ptr(pos, torch.float32, "pos"), B, np_, D, float(eps),
+                                       _ptr(gamma, torch.float32, "gamma"), _ptr(beta, torch.float32, "beta"),
+                                       _ptr(out, torch.float32, "out"), _stream()), "svi_quality_embed_ln")
+    return out
+
+
+def quality_quick_gelu(x, out):
+    """out bf16 = x * sigmoid(1.702 x) of x f32 (svi_quality_quick_gelu); both [M, N] row-major views."""
+    ldx, ldy = _rowmajor(x, "x"), _rowmajor(out, "out")
+    if x.shape != out.shape:
+        raise RuntimeError("svi_b200.quality_quick_gelu: x and out must have the same shape")
+    _check(load().svi_quality_quick_gelu(_ptr(x, torch.float32, "x"), ldx, x.shape[0], x.shape[1],
+                                         _ptr(out, torch.bfloat16, "out"), ldy, _stream()), "svi_quality_quick_gelu")
+    return out
+
+
+def quality_pool(x, n_seq, out, mode=POOL_FIRST, ids=None, eos_id=0):
+    """out f32 [n_seq, D] = one row per sequence of x f32 [n_seq * L, D] (svi_quality_pool): row 0, the argmax of ids
+    (int64 [n_seq, L]) or the first row whose id is eos_id."""
+    ldx = _rowmajor(x, "x")
+    if n_seq < 1 or x.shape[0] % n_seq or tuple(out.shape) != (n_seq, x.shape[1]) or not out.is_contiguous():
+        raise RuntimeError("svi_b200.quality_pool: x must hold n_seq sequences and out be a contiguous [n_seq, D] tensor")
+    L = x.shape[0] // n_seq
+    if ids is not None and (ids.dtype != torch.int64 or tuple(ids.shape) != (n_seq, L) or not ids.is_contiguous()):
+        raise RuntimeError(f"svi_b200.quality_pool: ids must be contiguous int64 [{n_seq}, {L}]")
+    _check(load().svi_quality_pool(_ptr(x, torch.float32, "x"), ldx, n_seq, L, x.shape[1], _ptr(ids, name="ids"), int(mode),
+                                   int(eos_id), _ptr(out, torch.float32, "out"), _stream()), "svi_quality_pool")
+    return out
+
+
+def quality_score(img, txt=None, cos=None, w=None, bias=0.0, aes=None):
+    """cos f32 [B, T] = normalised img [B, E] . normalised txt [T, E]; aes f32 [B] = w . normalised img + bias
+    (svi_quality_score)."""
+    B, E = img.shape
+    T = 0 if txt is None else txt.shape[0]
+    for t, n, shape in ((img, "img", (B, E)), (txt, "txt", (T, E)), (cos, "cos", (B, T)), (w, "w", (E,)), (aes, "aes", (B,))):
+        if t is not None and (tuple(t.shape) != shape or not t.is_contiguous()):
+            raise RuntimeError(f"svi_b200.quality_score: {n} must be a contiguous {shape} tensor, got {tuple(t.shape)}")
+    _check(load().svi_quality_score(_ptr(img, torch.float32, "img"), B, _ptr(txt, torch.float32, "txt"), T, E,
+                                    _ptr(w, torch.float32, "w"), float(bias), _ptr(cos, torch.float32, "cos"),
+                                    _ptr(aes, torch.float32, "aes"), _stream()), "svi_quality_score")
+    return cos, aes
