@@ -1,16 +1,20 @@
 // Image-text quality scoring: the CLIP towers' batched short-sequence attention and their staging, pooling and scoring
-// kernels (include/svi_b200_quality.h).  The projections and MLPs are svi_gemm_bf16 calls, the block LayerNorms
-// svi_layernorm_modulate.
+// kernels (include/svi_b200_quality.h), and the same attention with separate query / key lengths, a shared K/V head and a
+// key mask for the cross-attention scorers (svi_reward_attn, include/svi_b200_reward.h).  The projections and MLPs are
+// svi_gemm_bf16 calls, the block LayerNorms svi_layernorm_modulate.
 //
 // Attention.  One CTA of four warps takes 64 query rows of one head of one sequence; the grid covers every sequence and
 // head of a layer in one launch.  K and V^T of the sequence's first `kv_len` keys are staged in shared memory once, both
 // as K-major wgmma B operands in core-matrix order (no swizzle); the warpgroup keeps its 64 query rows as register A
 // fragments (wgmma RS form) and walks the keys in chunks of 64 with an online softmax (fp32 max and sum, bf16 P, which
 // goes back into wgmma as the register A operand of P V).  Causal CTAs stage and visit only the keys up to their last
-// query row.
+// query row.  With a key mask, masked keys get a score of -inf like keys past Lk; a query row whose keys seen so far are
+// all masked keeps a running max of -inf, and its rescale factors and probabilities are taken against 0 instead (they
+// are all 0), so a fully masked chunk ahead of the first kept key contributes nothing.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "../../include/svi_b200_quality.h"
+#include "../../include/svi_b200_reward.h"
 
 namespace svi {
 namespace quality {
@@ -57,29 +61,36 @@ __host__ __device__ constexpr int round_up(int x, int m) { return (x + m - 1) / 
 
 template <int HD>
 __host__ __device__ constexpr size_t attn_smem_bytes(int kv_pad) {
-  return (size_t)kv_pad * HD * 2 * 2;     // K [kv_pad][HD] and V^T [HD][kv_pad], bf16
+  return (size_t)kv_pad * HD * 2 * 2 + kv_pad;   // K [kv_pad][HD] and V^T [HD][kv_pad], bf16; the key mask, one byte a key
 }
 
+// Sequence b: query rows [b*Lq, (b+1)*Lq) of Q and O, key rows [b*kv_stride, b*kv_stride + Lk) of K and V, query head h
+// reading K/V head h (kv_shared == 0) or 0 (kv_shared != 0), mask bytes mask[b*mask_stride + key] (mask may be null).
 template <int HD>
 __global__ void __launch_bounds__(kAttnThreads)
 attn_kernel(const __nv_bfloat16* __restrict__ Q, long long ldq, const __nv_bfloat16* __restrict__ K, long long ldk,
-            const __nv_bfloat16* __restrict__ V, long long ldv, __nv_bfloat16* __restrict__ O, long long ldo, int L,
+            const __nv_bfloat16* __restrict__ V, long long ldv, __nv_bfloat16* __restrict__ O, long long ldo, int Lq,
+            int Lk, long long kv_stride, int kv_shared, const uint8_t* __restrict__ mask, long long mask_stride,
             float scale_log2, int causal) {
   extern __shared__ __align__(128) unsigned char smem[];
   const int q0 = blockIdx.x * kBQ, h = blockIdx.y, b = blockIdx.z;
-  const int kv_len = causal ? min(L, q0 + kBQ) : L;
+  const int kv_len = causal ? min(Lk, q0 + kBQ) : Lk;
   const int kv_pad = round_up(kv_len, kBK);
   unsigned char* Ks = smem;                                  // (n = key, k = d), K-major
   unsigned char* Vt = smem + (size_t)kv_pad * HD * 2;        // (n = d, k = key), K-major
-  const long long row0 = (long long)b * L;
+  unsigned char* Ms = smem + (size_t)kv_pad * HD * 4;        // 1 = key kept
+  const long long row0 = (long long)b * Lq, krow0 = (long long)b * kv_stride;
+  const int hk = kv_shared ? 0 : h;
 
+  if (mask != nullptr)
+    for (int j = threadIdx.x; j < kv_len; j += kAttnThreads) Ms[j] = mask[b * mask_stride + j] != 0;
   // stage K and V^T in core-matrix order; keys [kv_len, kv_pad) are zero (their P is zero, and 0 * garbage could be NaN)
   for (int i = threadIdx.x; i < kv_pad * (HD / 2); i += kAttnThreads) {
     const int j = i / (HD / 2), c = (i % (HD / 2)) * 2;
     uint32_t kw = 0u, vw = 0u;
     if (j < kv_len) {
-      kw = *reinterpret_cast<const uint32_t*>(K + (row0 + j) * ldk + h * HD + c);
-      vw = *reinterpret_cast<const uint32_t*>(V + (row0 + j) * ldv + h * HD + c);
+      kw = *reinterpret_cast<const uint32_t*>(K + (krow0 + j) * ldk + hk * HD + c);
+      vw = *reinterpret_cast<const uint32_t*>(V + (krow0 + j) * ldv + hk * HD + c);
     }
     *reinterpret_cast<uint32_t*>(Ks + cm_offset(j, c, HD)) = kw;
     const __nv_bfloat162 v2 = *reinterpret_cast<const __nv_bfloat162*>(&vw);
@@ -89,7 +100,7 @@ attn_kernel(const __nv_bfloat16* __restrict__ Q, long long ldq, const __nv_bfloa
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> wgmma operand reads
   __syncthreads();
 
-  // every warp runs every chunk (wgmma is warpgroup-wide); rows past L compute on zero Q and store nothing
+  // every warp runs every chunk (wgmma is warpgroup-wide); rows past Lq compute on zero Q and store nothing
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32, g = lane / 4, t = lane % 4;
   const int r_lo = q0 + warp * 16 + g, r_hi = r_lo + 8;
 
@@ -97,10 +108,10 @@ attn_kernel(const __nv_bfloat16* __restrict__ Q, long long ldq, const __nv_bfloa
 #pragma unroll
   for (int kk = 0; kk < HD / 16; ++kk) {
     const int c = h * HD + kk * 16 + t * 2;
-    qf[kk][0] = r_lo < L ? *reinterpret_cast<const uint32_t*>(Q + (row0 + r_lo) * ldq + c) : 0u;
-    qf[kk][1] = r_hi < L ? *reinterpret_cast<const uint32_t*>(Q + (row0 + r_hi) * ldq + c) : 0u;
-    qf[kk][2] = r_lo < L ? *reinterpret_cast<const uint32_t*>(Q + (row0 + r_lo) * ldq + c + 8) : 0u;
-    qf[kk][3] = r_hi < L ? *reinterpret_cast<const uint32_t*>(Q + (row0 + r_hi) * ldq + c + 8) : 0u;
+    qf[kk][0] = r_lo < Lq ? *reinterpret_cast<const uint32_t*>(Q + (row0 + r_lo) * ldq + c) : 0u;
+    qf[kk][1] = r_hi < Lq ? *reinterpret_cast<const uint32_t*>(Q + (row0 + r_hi) * ldq + c) : 0u;
+    qf[kk][2] = r_lo < Lq ? *reinterpret_cast<const uint32_t*>(Q + (row0 + r_lo) * ldq + c + 8) : 0u;
+    qf[kk][3] = r_hi < Lq ? *reinterpret_cast<const uint32_t*>(Q + (row0 + r_hi) * ldq + c + 8) : 0u;
   }
 
   float o[HD / 2];
@@ -128,8 +139,9 @@ attn_kernel(const __nv_bfloat16* __restrict__ Q, long long ldq, const __nv_bfloa
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const int key = kc * kBK + n * 8 + t * 2 + e;
-        if (key >= L || (causal && key > r_lo)) s[4 * n + e] = -INFINITY;
-        if (key >= L || (causal && key > r_hi)) s[4 * n + 2 + e] = -INFINITY;
+        const bool dropped = key >= Lk || (mask != nullptr && !Ms[key]);
+        if (dropped || (causal && key > r_lo)) s[4 * n + e] = -INFINITY;
+        if (dropped || (causal && key > r_hi)) s[4 * n + 2 + e] = -INFINITY;
         cm_lo = fmaxf(cm_lo, s[4 * n + e]);
         cm_hi = fmaxf(cm_hi, s[4 * n + 2 + e]);
       }
@@ -139,9 +151,11 @@ attn_kernel(const __nv_bfloat16* __restrict__ Q, long long ldq, const __nv_bfloa
       cm_lo = fmaxf(cm_lo, __shfl_xor_sync(0xffffffffu, cm_lo, off));
       cm_hi = fmaxf(cm_hi, __shfl_xor_sync(0xffffffffu, cm_hi, off));
     }
-    // key 0 is in chunk 0 and never masked, so the running max is finite from the first chunk on
+    // without a key mask, key 0 is in chunk 0 and never masked, so the running max is finite from the first chunk on and
+    // the reference point below is the running max itself
     const float mn_lo = fmaxf(m_lo, cm_lo), mn_hi = fmaxf(m_hi, cm_hi);
-    const float a_lo = exp2f((m_lo - mn_lo) * scale_log2), a_hi = exp2f((m_hi - mn_hi) * scale_log2);
+    const float ref_lo = mn_lo == -INFINITY ? 0.f : mn_lo, ref_hi = mn_hi == -INFINITY ? 0.f : mn_hi;
+    const float a_lo = exp2f((m_lo - ref_lo) * scale_log2), a_hi = exp2f((m_hi - ref_hi) * scale_log2);
     m_lo = mn_lo;
     m_hi = mn_hi;
     l_lo *= a_lo;
@@ -153,8 +167,8 @@ attn_kernel(const __nv_bfloat16* __restrict__ Q, long long ldq, const __nv_bfloa
     uint32_t pa[kBK / 16][4];
 #pragma unroll
     for (int n = 0; n < kBK / 8; ++n) {
-      const float p0 = exp2f((s[4 * n] - m_lo) * scale_log2), p1 = exp2f((s[4 * n + 1] - m_lo) * scale_log2);
-      const float p2 = exp2f((s[4 * n + 2] - m_hi) * scale_log2), p3 = exp2f((s[4 * n + 3] - m_hi) * scale_log2);
+      const float p0 = exp2f((s[4 * n] - ref_lo) * scale_log2), p1 = exp2f((s[4 * n + 1] - ref_lo) * scale_log2);
+      const float p2 = exp2f((s[4 * n + 2] - ref_hi) * scale_log2), p3 = exp2f((s[4 * n + 3] - ref_hi) * scale_log2);
       l_lo += p0 + p1;
       l_hi += p2 + p3;
       pa[n / 2][(n & 1) * 2] = pack_bf16x2(p0, p1);
@@ -178,29 +192,31 @@ attn_kernel(const __nv_bfloat16* __restrict__ Q, long long ldq, const __nv_bfloa
 #pragma unroll
   for (int n = 0; n < HD / 8; ++n) {
     const int c = h * HD + n * 8 + t * 2;
-    if (r_lo < L) *reinterpret_cast<uint32_t*>(O + (row0 + r_lo) * ldo + c) = pack_bf16x2(o[4 * n] * inv_lo, o[4 * n + 1] * inv_lo);
-    if (r_hi < L) *reinterpret_cast<uint32_t*>(O + (row0 + r_hi) * ldo + c) = pack_bf16x2(o[4 * n + 2] * inv_hi, o[4 * n + 3] * inv_hi);
+    if (r_lo < Lq) *reinterpret_cast<uint32_t*>(O + (row0 + r_lo) * ldo + c) = pack_bf16x2(o[4 * n] * inv_lo, o[4 * n + 1] * inv_lo);
+    if (r_hi < Lq) *reinterpret_cast<uint32_t*>(O + (row0 + r_hi) * ldo + c) = pack_bf16x2(o[4 * n + 2] * inv_hi, o[4 * n + 3] * inv_hi);
   }
 }
 
 template <int HD>
-int launch_attn(const void* Q, int64_t ldq, const void* K, int64_t ldk, const void* V, int64_t ldv, void* O, int64_t ldo,
-                int batch, int L, int heads, float scale, int causal, cudaStream_t stream) {
+int launch_attn(const char* name, const void* Q, int64_t ldq, const void* K, int64_t ldk, const void* V, int64_t ldv,
+                void* O, int64_t ldo, int batch, int Lq, int Lk, int heads, int64_t kv_stride, int kv_shared,
+                const uint8_t* mask, int64_t mask_stride, float scale, int causal, cudaStream_t stream) {
   static bool attr_set = false;       // the largest plan's shared memory, allowed once per process
   if (!attr_set) {
     const cudaError_t e = cudaFuncSetAttribute(attn_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                (int)attn_smem_bytes<HD>(round_up(SVI_QUALITY_MAX_L, kBK)));
     if (e != cudaSuccess) {
-      set_last_error("svi_quality_attn: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
+      set_last_error("%s: cudaFuncSetAttribute failed: %s", name, cudaGetErrorString(e));
       return SVI_ERR_DRIVER;
     }
     attr_set = true;
   }
-  const dim3 grid((unsigned)((L + kBQ - 1) / kBQ), (unsigned)heads, (unsigned)batch);
-  attn_kernel<HD><<<grid, kAttnThreads, attn_smem_bytes<HD>(round_up(L, kBK)), stream>>>(
+  const dim3 grid((unsigned)((Lq + kBQ - 1) / kBQ), (unsigned)heads, (unsigned)batch);
+  attn_kernel<HD><<<grid, kAttnThreads, attn_smem_bytes<HD>(round_up(Lk, kBK)), stream>>>(
       static_cast<const __nv_bfloat16*>(Q), ldq, static_cast<const __nv_bfloat16*>(K), ldk,
-      static_cast<const __nv_bfloat16*>(V), ldv, static_cast<__nv_bfloat16*>(O), ldo, L, scale * 1.4426950408889634f, causal);
-  SVI_CUDA_LAUNCH_CHECK("svi_quality_attn");
+      static_cast<const __nv_bfloat16*>(V), ldv, static_cast<__nv_bfloat16*>(O), ldo, Lq, Lk, (long long)kv_stride,
+      kv_shared, mask, (long long)mask_stride, scale * 1.4426950408889634f, causal);
+  SVI_CUDA_LAUNCH_CHECK(name);
   return SVI_OK;
 }
 
@@ -362,8 +378,38 @@ extern "C" int svi_quality_attn(const void* Q, int64_t ldq, const void* K, int64
   SVI_REQUIRE(!overlap(O, bo, Q, ((rows - 1) * ldq + w) * 2) && !overlap(O, bo, K, ((rows - 1) * ldk + w) * 2) &&
               !overlap(O, bo, V, ((rows - 1) * ldv + w) * 2), "svi_quality_attn: O overlaps Q, K or V");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  return head_dim == 64 ? launch_attn<64>(Q, ldq, K, ldk, V, ldv, O, ldo, batch, L, num_heads, scale, causal != 0, st)
-                        : launch_attn<80>(Q, ldq, K, ldk, V, ldv, O, ldo, batch, L, num_heads, scale, causal != 0, st);
+  const char* name = "svi_quality_attn";
+  return head_dim == 64 ? launch_attn<64>(name, Q, ldq, K, ldk, V, ldv, O, ldo, batch, L, L, num_heads, L, 0, nullptr, 0,
+                                          scale, causal != 0, st)
+                        : launch_attn<80>(name, Q, ldq, K, ldk, V, ldv, O, ldo, batch, L, L, num_heads, L, 0, nullptr, 0,
+                                          scale, causal != 0, st);
+}
+
+extern "C" int svi_reward_attn(const void* Q, int64_t ldq, const void* K, int64_t ldk, const void* V, int64_t ldv, void* O,
+                               int64_t ldo, int32_t batch, int32_t Lq, int32_t Lk, int32_t num_heads, int32_t kv_heads,
+                               int64_t kv_batch_stride, const uint8_t* key_mask, int64_t mask_batch_stride, float scale,
+                               void* stream) {
+  SVI_REQUIRE(Q && K && V && O, "svi_reward_attn: null pointer");
+  SVI_REQUIRE(Lq >= 1 && Lq <= SVI_QUALITY_MAX_L && Lk >= 1 && Lk <= SVI_QUALITY_MAX_L,
+              "svi_reward_attn: Lq = %d / Lk = %d outside [1, %d]", Lq, Lk, SVI_QUALITY_MAX_L);
+  SVI_REQUIRE(batch >= 1 && batch <= 65535 && num_heads >= 1 && num_heads <= 65535,
+              "svi_reward_attn: batch %d / num_heads %d outside [1, 65535]", batch, num_heads);
+  SVI_REQUIRE(kv_heads == 1 || kv_heads == num_heads, "svi_reward_attn: kv_heads %d must be 1 or num_heads", kv_heads);
+  SVI_REQUIRE(kv_batch_stride == 0 || kv_batch_stride >= Lk, "svi_reward_attn: kv_batch_stride must be 0 or >= Lk");
+  SVI_REQUIRE(mask_batch_stride == 0 || mask_batch_stride >= Lk, "svi_reward_attn: mask_batch_stride must be 0 or >= Lk");
+  const int64_t wq = (int64_t)num_heads * 64, wk = (int64_t)kv_heads * 64;
+  SVI_REQUIRE(ldq >= wq && ldo >= wq && ldk >= wk && ldv >= wk,
+              "svi_reward_attn: a leading dimension is below the heads' width (q, o: %lld; k, v: %lld)", (long long)wq,
+              (long long)wk);
+  SVI_REQUIRE(ldq % 2 == 0 && ldk % 2 == 0 && ldv % 2 == 0 && ldo % 2 == 0, "svi_reward_attn: leading dimensions must be even");
+  SVI_REQUIRE(aligned(Q, 4) && aligned(K, 4) && aligned(V, 4) && aligned(O, 4), "svi_reward_attn: pointers must be 4-byte aligned");
+  SVI_REQUIRE(scale > 0.f && scale < 1e30f, "svi_reward_attn: scale must be positive and finite");
+  const size_t q_rows = (size_t)batch * Lq, k_rows = (size_t)(kv_batch_stride * (batch - 1) + Lk);
+  const size_t bo = ((q_rows - 1) * ldo + wq) * 2;
+  SVI_REQUIRE(!overlap(O, bo, Q, ((q_rows - 1) * ldq + wq) * 2) && !overlap(O, bo, K, ((k_rows - 1) * ldk + wk) * 2) &&
+              !overlap(O, bo, V, ((k_rows - 1) * ldv + wk) * 2), "svi_reward_attn: O overlaps Q, K or V");
+  return launch_attn<64>("svi_reward_attn", Q, ldq, K, ldk, V, ldv, O, ldo, batch, Lq, Lk, num_heads, kv_batch_stride,
+                         kv_heads == 1, key_mask, mask_batch_stride, scale, 0, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int svi_quality_stage_pixels(const float* px, int32_t B, int32_t S, int32_t P, const float* mean_std, void* out,

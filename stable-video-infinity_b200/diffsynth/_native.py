@@ -1,7 +1,7 @@
 """ctypes binding of the C-ABI kernel library ``libsvi_b200.so`` (declared in ``include/svi_b200.h``,
 ``include/svi_b200_lora.h``, ``include/svi_b200_rife.h``, ``include/svi_b200_esrgan.h``,
-``include/svi_b200_fastblend.h``, ``include/svi_b200_unianimate.h``, ``include/svi_b200_replace.h`` and
-``include/svi_b200_quality.h``).
+``include/svi_b200_fastblend.h``, ``include/svi_b200_unianimate.h``, ``include/svi_b200_replace.h``,
+``include/svi_b200_quality.h`` and ``include/svi_b200_reward.h``).
 
 This is the only door between the Python host code and the hand-written sm_90a kernels.  There is no
 fallback: if the shared library is missing or a call fails, a ``RuntimeError`` is raised.
@@ -242,6 +242,18 @@ QUALITY_SIGNATURES = {
 QUALITY_MAX_L = 320
 POOL_FIRST, POOL_ARGMAX, POOL_EOS = 0, 1, 2
 
+# the same for include/svi_b200_reward.h
+REWARD_SIGNATURES = {
+    "svi_reward_attn": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _i64, _vp, _i64,
+                               _f32, _vp]),
+    "svi_reward_layernorm": (_i32, [_vp, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _vp]),
+    "svi_reward_embed": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
+    "svi_reward_swiglu": (_i32, [_vp, _i64, _i32, _i32, _vp, _i64, _vp]),
+    "svi_reward_rope": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "svi_reward_cond_mask": (_i32, [_vp, _i32, _vp, _i32, _i32, _f32, _vp, _vp, _vp]),
+    "svi_reward_head": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _f32, _vp, _vp]),
+}
+
 _lib = None
 
 
@@ -260,7 +272,8 @@ def load():
             f"`python -c 'import __graft_entry__ as g; g.build()'` (or `make`) — there is no CPU fallback.")
     lib = ctypes.CDLL(_LIB_PATH)
     for name, (res, args) in (SIGNATURES | LORA_SIGNATURES | RIFE_SIGNATURES | ESRGAN_SIGNATURES |
-                        FASTBLEND_SIGNATURES | UNIANIMATE_SIGNATURES | REPLACE_SIGNATURES | QUALITY_SIGNATURES).items():
+                        FASTBLEND_SIGNATURES | UNIANIMATE_SIGNATURES | REPLACE_SIGNATURES | QUALITY_SIGNATURES |
+                        REWARD_SIGNATURES).items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing: fail loudly
         fn.restype = res
         fn.argtypes = args
@@ -1260,3 +1273,100 @@ def quality_score(img, txt=None, cos=None, w=None, bias=0.0, aes=None):
                                     _ptr(w, torch.float32, "w"), float(bias), _ptr(cos, torch.float32, "cos"),
                                     _ptr(aes, torch.float32, "aes"), _stream()), "svi_quality_score")
     return cos, aes
+
+
+# --------------------------------------------------------------------------------------------- cross-attention scorers (include/svi_b200_reward.h)
+def reward_attn(q, k, v, out, batch, num_heads, scale, kv_heads=None, kv_shared=False, key_mask=None):
+    """softmax(q k^T * scale, masked keys excluded) v, head width 64 (svi_reward_attn).  q, out bf16 [batch * Lq, >= 64 H]
+    and k, v bf16 [batch * Lk (or Lk when kv_shared), >= 64 kv_heads] row-major views; kv_heads is num_heads (default) or
+    1.  key_mask uint8 [batch, Lk], or [1, Lk] / [Lk] shared by every sequence."""
+    ldq, ldk, ldv, ldo = (_rowmajor(t, n) for t, n in ((q, "q"), (k, "k"), (v, "v"), (out, "out")))
+    kv_heads = num_heads if kv_heads is None else kv_heads
+    rows = q.shape[0]
+    if batch < 1 or rows % batch or out.shape[0] != rows or k.shape[0] != v.shape[0] or (not kv_shared and k.shape[0] % batch):
+        raise RuntimeError(f"svi_b200.reward_attn: q / out rows must be a multiple of batch = {batch} and k, v agree")
+    Lq = rows // batch
+    Lk = k.shape[0] if kv_shared else k.shape[0] // batch
+    mstride = 0
+    if key_mask is not None:
+        if key_mask.dtype != torch.uint8 or not key_mask.is_contiguous() or key_mask.shape[-1] != Lk or \
+                key_mask.numel() not in (Lk, batch * Lk):
+            raise RuntimeError(f"svi_b200.reward_attn: key_mask must be contiguous uint8 [{batch}, {Lk}] or [{Lk}]")
+        mstride = Lk if key_mask.numel() == batch * Lk and batch > 1 else 0
+    _check(load().svi_reward_attn(_ptr(q, torch.bfloat16, "q"), ldq, _ptr(k, torch.bfloat16, "k"), ldk,
+                                  _ptr(v, torch.bfloat16, "v"), ldv, _ptr(out, torch.bfloat16, "out"), ldo, int(batch), Lq, Lk,
+                                  int(num_heads), int(kv_heads), 0 if kv_shared else Lk, _ptr(key_mask, torch.uint8, "key_mask"),
+                                  mstride, float(scale), _stream()), "svi_reward_attn")
+    return out
+
+
+def reward_layernorm(x, gamma, beta, eps, y, yb):
+    """y f32 = LN(x) * gamma + beta (y may be x) and yb bf16 = the same values rounded (svi_reward_layernorm)."""
+    M, D = x.shape
+    if not (x.is_contiguous() and y.is_contiguous() and yb.is_contiguous()) or y.shape != x.shape or yb.shape != x.shape:
+        raise RuntimeError("svi_b200.reward_layernorm: x, y, yb must be contiguous and of one shape")
+    _check(load().svi_reward_layernorm(_ptr(x, torch.float32, "x"), M, D, float(eps), _ptr(gamma, torch.float32, "gamma"),
+                                       _ptr(beta, torch.float32, "beta"), _ptr(y, torch.float32, "y"),
+                                       _ptr(yb, torch.bfloat16, "yb"), _stream()), "svi_reward_layernorm")
+    return y, yb
+
+
+def reward_embed(patch, cls, pos, out):
+    """out f32 [B*(1+np), D] = [cls; patch rows of image b] + pos per image (svi_reward_embed)."""
+    np_, D = pos.shape[0] - 1, pos.shape[1]
+    if patch.dim() != 2 or patch.shape[1] != D or patch.shape[0] % np_ or not patch.is_contiguous() or not pos.is_contiguous():
+        raise RuntimeError("svi_b200.reward_embed: patch must be a contiguous [B * np, D] tensor")
+    B = patch.shape[0] // np_
+    if tuple(out.shape) != (B * (np_ + 1), D) or not out.is_contiguous() or cls.numel() != D:
+        raise RuntimeError("svi_b200.reward_embed: out must be a contiguous [B * (np + 1), D] tensor and cls hold D floats")
+    _check(load().svi_reward_embed(_ptr(patch, torch.float32, "patch"), _ptr(cls, torch.float32, "cls"),
+                                   _ptr(pos, torch.float32, "pos"), B, np_, D, _ptr(out, torch.float32, "out"), _stream()),
+           "svi_reward_embed")
+    return out
+
+
+def reward_swiglu(x, out):
+    """out bf16 [M, F] = silu(g) * a of x f32 [M, 2F] = [a | g] (svi_reward_swiglu); row-major views."""
+    ldx, ldy = _rowmajor(x, "x"), _rowmajor(out, "out")
+    M, F2 = x.shape
+    if F2 % 2 or tuple(out.shape) != (M, F2 // 2):
+        raise RuntimeError("svi_b200.reward_swiglu: x must be [M, 2F] and out [M, F]")
+    _check(load().svi_reward_swiglu(_ptr(x, torch.float32, "x"), ldx, M, F2 // 2, _ptr(out, torch.bfloat16, "out"), ldy,
+                                    _stream()), "svi_reward_swiglu")
+    return out
+
+
+def reward_rope(x, L, cos, sin):
+    """rotate-half RoPE in place on the 64-wide heads of x bf16 [M, 64 heads] (row-major view), position = row % L;
+    cos, sin f32 [L, 32] (svi_reward_rope)."""
+    ldx = _rowmajor(x, "x")
+    M, W = x.shape
+    if W % 64 or tuple(cos.shape) != (L, 32) or tuple(sin.shape) != (L, 32) or not (cos.is_contiguous() and sin.is_contiguous()):
+        raise RuntimeError("svi_b200.reward_rope: x must be [M, 64 * heads] and cos, sin contiguous [L, 32]")
+    _check(load().svi_reward_rope(_ptr(x, torch.bfloat16, "x"), ldx, M, int(L), W // 64, _ptr(cos, torch.float32, "cos"),
+                                  _ptr(sin, torch.float32, "sin"), _stream()), "svi_reward_rope")
+    return x
+
+
+def reward_cond_mask(text, cond, threshold, ratio, keep):
+    """ratio f32 [Lt] = max_j text[i] . cond[j] over its maximum, keep uint8 [Lt] = ratio > threshold
+    (svi_reward_cond_mask); text f32 [Lt, E], cond f32 [Lc, E]."""
+    (Lt, E), Lc = text.shape, cond.shape[0]
+    if not (text.is_contiguous() and cond.is_contiguous() and ratio.is_contiguous() and keep.is_contiguous()) or \
+            cond.shape[1] != E or ratio.numel() != Lt or keep.numel() != Lt:
+        raise RuntimeError("svi_b200.reward_cond_mask: contiguous text [Lt, E], cond [Lc, E], ratio and keep [Lt] required")
+    _check(load().svi_reward_cond_mask(_ptr(text, torch.float32, "text"), Lt, _ptr(cond, torch.float32, "cond"), Lc, E,
+                                       float(threshold), _ptr(ratio, torch.float32, "ratio"), _ptr(keep, torch.uint8, "keep"),
+                                       _stream()), "svi_reward_cond_mask")
+    return ratio, keep
+
+
+def reward_head(x, n_seq, w, bias, out):
+    """out f32 [n_seq] = w . (row 0 of each sequence of x f32 [n_seq * L, E]) + bias (svi_reward_head)."""
+    ldx = _rowmajor(x, "x")
+    if n_seq < 1 or x.shape[0] % n_seq or w.numel() != x.shape[1] or out.numel() != n_seq or not out.is_contiguous():
+        raise RuntimeError("svi_b200.reward_head: x must hold n_seq sequences, w E floats and out n_seq floats")
+    _check(load().svi_reward_head(_ptr(x, torch.float32, "x"), ldx, n_seq, x.shape[0] // n_seq, x.shape[1],
+                                  _ptr(w, torch.float32, "w"), float(bias), _ptr(out, torch.float32, "out"), _stream()),
+           "svi_reward_head")
+    return out

@@ -22,4 +22,6 @@ MODEL_PATHS = {
     "mps": get_model_path("MPS_overall_checkpoint/MPS_overall_checkpoint_diffsynth.safetensors"),
     "pickscore": get_model_path("PickScore_v1"),
     "open_clip_bpe": get_model_path("bpe_simple_vocab_16e6.txt.gz"),
+    # ImageReward's tokenizer directory; the reference's dict lacks this key, so its default ImageRewardScore fails
+    "bert_model_path": get_model_path("bert-base-uncased"),
 }

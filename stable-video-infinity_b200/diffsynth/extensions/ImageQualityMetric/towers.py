@@ -23,6 +23,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+from PIL import Image
 
 from ... import _native as nv
 
@@ -276,15 +277,16 @@ class AestheticMLP(nn.Module):
         self.layers = nn.Sequential(nn.Linear(input_size, 1024), nn.Dropout(0.2), nn.Linear(1024, 128), nn.Dropout(0.2),
                                     nn.Linear(128, 64), nn.Dropout(0.1), nn.Linear(64, 16), nn.Linear(16, 1))
 
-    def folded(self):
-        """(w [input_size], b): the five layers composed on the host in fp64, rounded once to f32."""
+    def folded(self, shift=0.0, scale=1.0):
+        """(w [input_size], b) of (layers(x) - shift) / scale: the five layers and the standardisation composed on the host
+        in fp64, rounded once to f32."""
         w = torch.eye(self.layers[0].in_features, dtype=torch.float64)
         b = torch.zeros(self.layers[0].in_features, dtype=torch.float64)
         for i in (0, 2, 4, 6, 7):
             lin = self.layers[i]
             W = lin.weight.detach().double().cpu()
             w, b = W @ w, W @ b + lin.bias.detach().double().cpu()
-        return w[0].float(), float(b[0])
+        return (w[0] / scale).float(), float((b[0] - shift) / scale)
 
 
 # ================================================================================================ engines
@@ -304,7 +306,8 @@ class TowerSpec:
     patch: int = 0
     patch_weight: torch.Tensor = None
     cls: torch.Tensor = None
-    pre_ln: tuple = None
+    pre_ln: tuple = None            # None: no LayerNorm after the position embedding (BLIP's ViT)
+    patch_bias: torch.Tensor = None
     token_embedding: torch.Tensor = None
     pool: int = nv.POOL_FIRST
     eos_id: int = 0
@@ -312,7 +315,10 @@ class TowerSpec:
 
 class TowerEngine:
     """One CLIP tower on the device.  ``encode_images(px)`` takes preprocessed (un-normalised) f32 [B, 3, S, S] pixels,
-    ``encode_text(ids)`` int64 [T, L] token ids; both return the projected f32 features [n, embed_dim], not normalised."""
+    ``encode_text(ids)`` int64 [T, L] token ids; both return the projected f32 features [n, embed_dim], not normalised.
+    ``image_states(px)`` is the residual stream after the last block, every row of every image; ``encode_text_rows(ids)``
+    projects every row after the final LayerNorm and pools afterwards (the cross-attention scorers use both).  A tower
+    without a projection (``proj`` None) has only ``image_states``."""
 
     def __init__(self, spec, device, mean=OPENAI_MEAN, std=OPENAI_STD, chunk=128):
         nv.require_cuda(device, "the quality-metric towers")
@@ -328,8 +334,8 @@ class TowerEngine:
                        for b in spec.blocks]
         self.mlp_width = self.layers[0]["w_1"].shape[0]
         self.fw, self.fb = f32(spec.final_ln[0]), f32(spec.final_ln[1])
-        self.w_proj = bf(spec.proj)
-        self.embed_dim = self.w_proj.shape[0]
+        self.w_proj = bf(spec.proj) if spec.proj is not None else None
+        self.embed_dim = self.w_proj.shape[0] if spec.proj is not None else None
         self.pos = f32(spec.pos)
         if spec.patch_weight is not None:                  # vision tower
             P = self.patch = spec.patch
@@ -339,8 +345,9 @@ class TowerEngine:
             wp = torch.zeros(spec.width, self.kpad)
             wp[:, :k] = spec.patch_weight.detach().float().reshape(spec.width, k).cpu()
             self.w_patch = bf(wp)
+            self.b_patch = f32(spec.patch_bias) if spec.patch_bias is not None else None
             self.cls = f32(spec.cls)
-            self.pre_w, self.pre_b = f32(spec.pre_ln[0]), f32(spec.pre_ln[1])
+            self.pre_ln = (f32(spec.pre_ln[0]), f32(spec.pre_ln[1])) if spec.pre_ln is not None else None
             self.mean_std = torch.tensor([*mean, *std], dtype=torch.float32, device=self.device)
         else:
             self.tok = bf(spec.token_embedding)
@@ -382,27 +389,35 @@ class TowerEngine:
         self.launches += 3
         return feats
 
-    def encode_images(self, px):
-        B = px.shape[0]
+    def check_pixels(self, px):
         if tuple(px.shape[1:]) != (3, self.image_size, self.image_size):
             raise ValueError(f"ImageQualityMetric: pixels must be [B, 3, {self.image_size}, {self.image_size}], got {tuple(px.shape)}")
+
+    def encode_images(self, px):
+        B = px.shape[0]
+        self.check_pixels(px)
         out = torch.empty(B, self.embed_dim, device=self.device, dtype=torch.float32)
         for s in range(0, B, self.chunk):
-            out[s:s + self.chunk] = self._encode_image_chunk(px[s:s + self.chunk].to(self.device, torch.float32).contiguous())
+            chunk = px[s:s + self.chunk].to(self.device, torch.float32).contiguous()
+            out[s:s + self.chunk] = self._head(self.image_states(chunk), chunk.shape[0])
         return out
 
-    def _encode_image_chunk(self, px):
+    def image_states(self, px):
+        """preprocessed pixels f32 [B, 3, S, S] on the device (one chunk) -> residual stream f32 [B * (1 + np), width]"""
         dev, B, d = self.device, px.shape[0], self.width
         n = (self.image_size // self.patch) ** 2
         a = torch.empty(B * n, self.kpad, device=dev, dtype=torch.bfloat16)
         nv.quality_stage_pixels(px, self.mean_std, a, self.patch)
         patch = torch.empty(B * n, d, device=dev, dtype=torch.float32)
-        nv.gemm(a, self.w_patch, patch)
+        nv.gemm(a, self.w_patch, patch, bias=self.b_patch)
         x = torch.empty(B * (n + 1), d, device=dev, dtype=torch.float32)
-        nv.quality_embed_ln(patch, self.cls, self.pos, self.pre_w, self.pre_b, self.eps, x)
+        if self.pre_ln is not None:
+            nv.quality_embed_ln(patch, self.cls, self.pos, *self.pre_ln, self.eps, x)
+        else:
+            nv.reward_embed(patch, self.cls, self.pos, x)
         self.launches += 3
         self._blocks(x, B)
-        return self._head(x, B)
+        return x
 
     def encode_text(self, ids):
         dev, (T, L) = self.device, ids.shape
@@ -416,6 +431,27 @@ class TowerEngine:
         self.launches += 2
         self._blocks(x, T)
         return self._head(x, T, ids)
+
+    def encode_text_rows(self, ids):
+        """(every row after the final LayerNorm, projected: f32 [T * L, embed_dim]; the pooled rows of those, f32
+        [T, embed_dim]).  LayerNorm and projection act per row, so the pooled rows are the bytes encode_text returns."""
+        dev, (T, L) = self.device, ids.shape
+        if L > self.pos.shape[0]:
+            raise ValueError(f"ImageQualityMetric: {L} tokens exceed the text tower's {self.pos.shape[0]} positions")
+        ids = ids.to(device=dev, dtype=torch.int64).contiguous()
+        g = torch.empty(T * L, self.width, device=dev, dtype=torch.float32)
+        nv.embedding_gather(ids.view(-1), self.tok, g)
+        x = torch.empty_like(g)
+        nv.add_rows(g, self.pos[:L].contiguous(), x)
+        self._blocks(x, T)
+        hn = torch.empty(T * L, self.width, device=dev, dtype=torch.bfloat16)
+        nv.layernorm_modulate(x, hn, self.eps, gamma=self.fw, beta=self.fb)
+        rows = torch.empty(T * L, self.embed_dim, device=dev, dtype=torch.float32)
+        nv.gemm(hn, self.w_proj, rows)
+        pooled = torch.empty(T, self.embed_dim, device=dev, dtype=torch.float32)
+        nv.quality_pool(rows, T, pooled, self.pool, ids, self.eos_id)
+        self.launches += 6
+        return rows, pooled
 
 
 class CLIPEngines:
@@ -460,6 +496,23 @@ def openclip_pixels(image, size):
         ph, pw = size - nh, size - nw
         x = F.pad(x, (pw // 2, pw - pw // 2, ph // 2, ph - ph // 2), value=0.0)
     return x
+
+
+def blip_pixels(image, size):
+    """torchvision's Resize(size, BICUBIC) on the PIL image (the shorter side becomes `size`, the longer one
+    int(size * long / short); no resampling when the shorter side is already `size`), CenterCrop(size) (offsets
+    int(round((side - size) / 2))), conversion to RGB, ToTensor: f32 [3, size, size] in [0, 1].  Normalisation runs on the
+    device."""
+    if image.mode == "RGBA":
+        to_rgb(image)
+    w, h = image.size
+    short, long = (w, h) if w <= h else (h, w)
+    nw, nh = (size, int(size * long / short)) if w <= h else (int(size * long / short), size)
+    if (nw, nh) != (w, h):
+        image = image.resize((nw, nh), Image.BICUBIC)
+    top, left = int(round((nh - size) / 2.0)), int(round((nw - size) / 2.0))
+    image = image.crop((left, top, left + size, top + size)).convert("RGB")
+    return torch.from_numpy(np.asarray(image, dtype=np.uint8).copy()).permute(2, 0, 1).float().div(255)
 
 
 def hf_pixels(processor, image):
