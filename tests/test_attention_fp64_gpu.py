@@ -124,21 +124,32 @@ def to_bf16(x, mode="rne"):
     return f.to(torch.bfloat16)
 
 
-def scores(q, k, cs):
-    """x = (q k^T) c_r in fp64, padded with -inf to whole K/V tiles: [R, n_kv, 128]"""
-    x = (q.double() @ k.double().t()) * cs[:, None]
-    n = _cdiv(k.shape[0], T)
-    return F.pad(x, (0, n * T - k.shape[0]), value=-math.inf).view(x.shape[0], n, T)
+def scores(q, k, cs, tile=T):
+    """x = (q k^T) c_r in fp64, padded with -inf to whole K/V tiles of `tile` keys: [R, n_kv, tile].  q [G, Lq, d] and
+    k [G, Lk, d] give the rows of G independent groups one after the other (R = G Lq); cs is [R] or a number."""
+    x = q.double() @ k.double().transpose(-1, -2)
+    x = x.reshape(-1, k.shape[-2])
+    x = x * (cs[:, None] if torch.is_tensor(cs) else cs)
+    Lk = k.shape[-2]
+    n = _cdiv(Lk, tile)
+    return F.pad(x, (0, n * tile - Lk), value=-math.inf).view(x.shape[0], n, tile)
+
+
+def _rows_at(w, v):
+    """w [R, Lk] times v: [Lk, d] shared by every row, or [G, Lk, d] for G groups of R / G rows each"""
+    if v.dim() == 2:
+        return w @ v
+    return (w.view(v.shape[0], -1, w.shape[1]) @ v).reshape(w.shape[0], v.shape[2])
 
 
 def exact_softmax(xt, v):
-    """(O*, (P|V|)/l) of the rows of xt"""
-    R, Lk = xt.shape[0], v.shape[0]
+    """(O*, (P|V|)/l) of the rows of xt; the chunk width is xt's last dimension and does not enter the result"""
+    R, Lk = xt.shape[0], v.shape[-2]
     x = xt.reshape(R, -1)[:, :Lk]
     e = torch.exp2(x - x.amax(1, keepdim=True))
     l = e.sum(1, keepdim=True)
     v = v.double()
-    return (e @ v) / l, (e @ v.abs()) / l
+    return _rows_at(e, v) / l, _rows_at(e, v.abs()) / l
 
 
 def running_max(xt, segments):
@@ -152,19 +163,21 @@ def running_max(xt, segments):
 
 
 def kernel_order(xt, v, segments, p_round="rne", rowsum="exact", eta=None):
-    """O_model of the rows of xt (p_round None: no rounding of P; "trunc": truncated), and with eta [R] the tie term of
-    bar B's floor: over the P within eta_r P of a bf16 rounding midpoint, t_j = (bf16 step of P_j) 2^(m_t - m) |v_j| / l,
-    combined as min(sum t_j, 3 sqrt(sum t_j^2)): the worst case while few such P are involved, three standard deviations
-    of a sum with independent signs when many are"""
-    R, Lk = xt.shape[0], v.shape[0]
+    """O_model of the rows of xt, visiting K/V tiles of xt.shape[2] keys (p_round None: no rounding of P; "trunc":
+    truncated), and with eta [R] the tie term of bar B's floor: over the P within eta_r P of a bf16 rounding midpoint,
+    t_j = (bf16 step of P_j) 2^(m_t - m) |v_j| / l, combined as min(sum t_j, 3 sqrt(sum t_j^2)): the worst case while few
+    such P are involved, three standard deviations of a sum with independent signs when many are.  v is [Lk, d] or
+    [G, Lk, d] (see _rows_at).  A row whose keys so far are all masked (x = -inf, running max -inf) takes its P and
+    alpha against 0, as svi_quality_attn does: they are exactly 0, so such tiles contribute nothing."""
+    R, Lk = xt.shape[0], v.shape[-2]
     v = v.double()
     M = running_max(xt, segments)
     sc = torch.exp2(M - M.amax(1, keepdim=True))[:, :, None]
-    P = torch.exp2(xt - M[:, :, None])
+    P = torch.exp2(xt - M.masked_fill(M == -math.inf, 0.0)[:, :, None])
     Pr = P if p_round is None else to_bf16(P, p_round).double()
     w = (Pr * sc).reshape(R, -1)[:, :Lk]
     l = (w if rowsum == "bf16" else (P * sc).reshape(R, -1)[:, :Lk]).sum(1, keepdim=True)
-    o = (w @ v) / l
+    o = _rows_at(w, v) / l
     if eta is None:
         return o, None
     b = P.float().view(torch.int32) & -65536
@@ -172,14 +185,14 @@ def kernel_order(xt, v, segments, p_round="rne", rowsum="exact", eta=None):
     near = (P - (lo + hi) / 2).abs() <= eta.view(R, 1, 1) * P
     amb = torch.where(near, (hi - lo) * sc, torch.zeros((), dtype=P.dtype, device=P.device)).reshape(R, -1)[:, :Lk]
     va = v.abs()
-    return o, torch.minimum(amb @ va, 3 * ((amb * amb) @ (va * va)).sqrt()) / l
+    return o, torch.minimum(_rows_at(amb, va), 3 * _rows_at(amb * amb, va * va).sqrt()) / l
 
 
 # ------------------------------------------------------------------------------------------------------------- bars
-def bar_a(got, ref, pv, eps):
-    """(elements outside, worst err/bound) of bar A"""
+def bar_a(got, ref, pv, eps, extra=0.0):
+    """(elements outside, worst err/bound) of bar A; `extra` is an absolute term added to the bound"""
     half = 0.5 * torch.maximum(_bf16_ulp(got.float()), _bf16_ulp(ref.float())).double()
-    bound = eps * pv + half + 2 * ULP32 * ref.abs()
+    bound = eps * pv + half + 2 * ULP32 * ref.abs() + extra
     err = (got.double() - ref).abs()
     inside = err <= bound
     ratio = torch.where(err == 0, torch.zeros_like(err), err / bound.clamp_min(1e-300))

@@ -169,6 +169,11 @@ def test_header_matches_signatures_and_gpu_cases():
     assert set(gpu.COVERED) == names
     for entry, cases in gpu.COVERED.items():
         assert cases and all(callable(getattr(gpu, c, None)) and c.startswith("test_") for c in cases), entry
+    import test_quality_fp64_gpu as fp64
+    assert set(fp64.COVERED) <= names | set(nv.REWARD_SIGNATURES), "the fp64 module names an undeclared entry point"
+    for entry, cases in fp64.COVERED.items():
+        if entry in names:
+            assert cases and all(callable(getattr(fp64, c, None)) and c.startswith("test_") for c in cases), entry
     for macro, value in (("SVI_QUALITY_MAX_L", nv.QUALITY_MAX_L), ("SVI_POOL_FIRST", nv.POOL_FIRST),
                          ("SVI_POOL_ARGMAX", nv.POOL_ARGMAX), ("SVI_POOL_EOS", nv.POOL_EOS)):
         assert re.search(rf"#define {macro} {value}\b", src), macro

@@ -187,6 +187,10 @@ def test_header_matches_signatures_and_gpu_cases():
     assert set(gpu.COVERED) == names
     for entry, cases in gpu.COVERED.items():
         assert cases and all(callable(getattr(gpu, c, None)) and c.startswith("test_") for c in cases), entry
+    import test_quality_fp64_gpu as fp64
+    for entry, cases in fp64.COVERED.items():
+        if entry in names:
+            assert cases and all(callable(getattr(fp64, c, None)) and c.startswith("test_") for c in cases), entry
     if os.path.exists(nv.lib_path()):
         lib = ctypes.CDLL(nv.lib_path())
         assert all(hasattr(lib, n) for n in names)
