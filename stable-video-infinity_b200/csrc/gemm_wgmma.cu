@@ -1,19 +1,19 @@
 // Persistent warp-specialised bf16 GEMM for sm_90a:  out = epilogue(A[M,K] @ W[N,K]^T).
 //
-//   warpgroup 0     : TMA producer (one lane; 128B-swizzled 128x64 A and 128x64 W tiles into a 6-stage ring), 40 registers
-//   warpgroups 1, 2 : consumers in ping-pong: each owns whole 128 x 128 tiles (the CTA's even and odd tiles), as two
-//                     m64n128k16 row halves with the fp32 accumulator in registers, then runs the epilogue straight from
-//                     those registers, 232 registers
+//   warpgroup 0     : TMA producer (one lane; 128B-swizzled 128x64 A and 256x64 W tiles into a 4-stage ring), 40 registers
+//   warpgroups 1, 2 : consumers sharing each 128 x 256 tile: warpgroup w takes rows [64 w, 64 w + 64) as one m64n256k16
+//                     per k16 step, fp32 accumulators in registers (128 per thread), then runs the epilogue straight from
+//                     those registers in two 128-column passes, 232 registers
 //
-// The ring is filled in tile order and each tile's k-blocks belong to one warpgroup; an ordering barrier hands the ring
-// from one warpgroup to the other after each mainloop, so the mainloops alternate: while one warpgroup runs its epilogue
-// (bias, activation, residual loads, stores), the other's MMAs keep the tensor cores busy.
+// The wide tile is for the operand feed: per k16 step each warpgroup reads the 256-row W slice from shared memory once for
+// 64 x 256 outputs, and a tile moves 48 KB of operands from L2 per 4.2 MFLOP.  Its epilogue does not overlap MMAs of the
+// same CTA; the producer keeps filling the ring with the next tile's k-blocks meanwhile.
 //
 // e4m3 weights (svi_gemm_epilogue.w_e4m3 = 1; the reference's weight-only FP8 mode): the producer lane TMA-loads the
-// 128 x 64 e4m3 W tile (8 KB, unswizzled) into a staging ring instead, and warps 1-3 of warpgroup 0 (idle in the bf16
+// 256 x 64 e4m3 W tile (16 KB, unswizzled) into a staging ring instead, and warps 1-3 of warpgroup 0 (idle in the bf16
 // instantiation) convert it, exactly, into the bf16 W tile in the same 128B-swizzled layout the bf16 TMA load produces.
 // The consumers, their wgmma descriptors and the epilogue are the same code, so the result is bit-identical to the bf16
-// GEMM on bf16(W).  Shared memory: 5 bf16 stages (160 KB) + 4 staging stages (32 KB), against 6 x 32 KB for bf16.
+// GEMM on bf16(W).  Shared memory: 4 bf16 stages (192 KB) + 2 staging stages (32 KB), against 4 x 48 KB for bf16.
 //
 // The producer runs ahead across tiles, so operand loads overlap the epilogues.  Tiles are visited in groups of GROUP_M
 // row blocks so that the CTAs resident together share A and W tiles in L2.
@@ -24,6 +24,8 @@
 // tile's column group) and B [N, R]; the consumers run them into the same accumulators, so every epilogue stage sees the
 // LoRA term.  Those tiles are bf16 in both weight formats: with e4m3 W the producer TMA-loads the B tile straight into the
 // swizzled W half and makes the converter warps' arrivals on the stage's full barrier itself; the converters step over it.
+// Column groups of an odd multiple of 128 would straddle a 256-column tile; svi_gemm_lora_bf16 launches those one group
+// at a time.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "../../include/svi_b200.h"
@@ -33,24 +35,26 @@ namespace svi {
 namespace gemm {
 
 constexpr int BM = 128;
-constexpr int BN = 128;
+constexpr int BN = 256;
+constexpr int EPI_N = 128;  // columns per epilogue pass (one 128-column half of a warp's accumulators)
 constexpr int BK = 64;  // 64 bf16 = 128 B = one swizzle row
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
-constexpr int B_STAGE_BYTES = BN * BK * 2;  // 16 KB
+constexpr int B_STAGE_BYTES = BN * BK * 2;  // 32 KB
 constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-constexpr int W8_STAGE_BYTES = BN * BK;     // 8 KB of e4m3 W
+constexpr int W8_STAGE_BYTES = BN * BK;     // 16 KB of e4m3 W
 constexpr int NUM_THREADS = 384;
 constexpr int NUM_CONVERTERS = 96;          // warps 1-3 of warpgroup 0 (e4m3 instantiation)
-constexpr int GROUP_M = 8;
+constexpr int GROUP_M = 8;                  // 16 measured no faster on 256-column tiles (DESIGN.md §4)
 constexpr int RES_J = 4;                    // 8-column blocks whose residual, bias and gate loads go out together
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 65536
 static_assert(A_STAGE_BYTES % 1024 == 0 && STAGE_BYTES % 1024 == 0, "operand tiles must stay 1024-byte aligned");
-static_assert((BN / 8) % RES_J == 0, "residual batches must tile the warp's columns");
+static_assert((EPI_N / 8) % RES_J == 0 && BN % EPI_N == 0, "residual batches must tile the warp's columns");
 
 // Ring depths per weight format: bf16 stages (A + bf16 W) and e4m3 staging stages.
 template <bool kE4M3> struct Rings;
-template <> struct Rings<false> { static constexpr int STAGES = 6, W8_STAGES = 0; };
-template <> struct Rings<true> { static constexpr int STAGES = 5, W8_STAGES = 4; };
+// 4 bf16 stages: 3 measured slower on ffn.0 / ffn.2 (DESIGN.md §4)
+template <> struct Rings<false> { static constexpr int STAGES = 4, W8_STAGES = 0; };
+template <> struct Rings<true> { static constexpr int STAGES = 4, W8_STAGES = 2; };
 template <bool kE4M3>
 constexpr int smem_bytes() {
   return Rings<kE4M3>::STAGES * STAGE_BYTES + Rings<kE4M3>::W8_STAGES * W8_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
@@ -77,7 +81,7 @@ __device__ __forceinline__ uint2 e4m3x4_to_bf16x4(uint32_t w) {
   return make_uint2(lo, hi);
 }
 
-// One 128 x 64 e4m3 staging tile (row-major, 64 B per row) -> the bf16 W tile as the 128B-swizzled TMA load lays it out:
+// One 256 x 64 e4m3 staging tile (row-major, 64 B per row) -> the bf16 W tile as the 128B-swizzled TMA load lays it out:
 // row r at byte 128 r, its 16-byte chunk j at chunk position j ^ (r & 7).  Thread t takes 16-byte source chunks t, t + 96, ...
 // (row i / 4, bf16 chunks 2 (i % 4) and 2 (i % 4) + 1); a quarter-warp's stores hit eight distinct bank groups.
 __device__ __forceinline__ void convert_w_tile(uint32_t src, uint32_t dst, int t) {
@@ -106,6 +110,7 @@ struct Epi {
   int sumsq_groups;
   int sumsq_group_cols;
   int sumsq_parts;
+  int sumsq_col0;          // the column that this launch's column 0 is in the row sums' column grouping
   // LayerNorm folded into this GEMM (consumer side): A holds bf16(x * g) of the UN-normalised rows x; with the row statistics
   // (sum x, sum x^2) the epilogue reconstructs  LN(x)*g + t  times W^T  =  r_m (acc - mu_m u_n) + c_n,  u = W g, c = W t + b
   // (c arrives as `bias`)
@@ -122,10 +127,10 @@ struct Epi {
 // The LoRA segment of a launch: empty in the plain instantiations, whose parameter list and code stay as they were.
 template <bool kLoRA> struct LoRAArgs {};
 template <> struct LoRAArgs<true> {
-  CUtensorMap u;    // U [M, groups R] bf16, 64 x 128 boxes, 128B swizzle
-  CUtensorMap b;    // B [N, R] bf16, same boxes
+  CUtensorMap u;    // U [M, groups R] bf16, 64 x 128 boxes (BM rows), 128B swizzle
+  CUtensorMap b;    // B [N, R] bf16, 64 x 256 boxes (BN rows), 128B swizzle
   int kb;           // R / BK
-  int group_cols;   // 0: one group
+  int group_cols;   // 0: one group; else a multiple of BN (svi_gemm_lora_bf16 launches narrower groups one by one)
 };
 
 __device__ __forceinline__ void mbar_arrive_cnt_a(uint32_t bar, uint32_t count) {
@@ -186,7 +191,7 @@ __device__ __forceinline__ void sumsq_flush(const Epi& ep, int row, bool ok, int
 // move a load above an earlier store: the residual, bias and gate loads of RES_J column blocks are issued together, ahead
 // of their stores, which makes one memory round trip per batch instead of one per column block.
 template <int kAct, bool kF32, bool kFold>
-__device__ __forceinline__ void epilogue(const Epi& ep, float (&acc)[BN / 2], int M, int N, int row0, int n_base, int lane) {
+__device__ __forceinline__ void epilogue(const Epi& ep, float (&acc)[EPI_N / 2], int M, int N, int row0, int n_base, int lane) {
   const int g = lane >> 2, c = lane & 3;
   const int rows[2] = {row0 + g, row0 + g + 8};
   const bool ok[2] = {rows[0] < M, rows[1] < M};
@@ -216,7 +221,7 @@ __device__ __forceinline__ void epilogue(const Epi& ep, float (&acc)[BN / 2], in
                       : (void*)(reinterpret_cast<__nv_bfloat16*>(ep.out) + rows[h] * ep.ldo + col0);
   }
 #pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
+  for (int j = 0; j < EPI_N / 8; ++j) {
     if (j % RES_J == 0) {
 #pragma unroll
       for (int i = 0; i < RES_J; ++i) {
@@ -235,7 +240,7 @@ __device__ __forceinline__ void epilogue(const Epi& ep, float (&acc)[BN / 2], in
     if (n0 < N) {   // warp-uniform (N % 8 == 0)
       const int n = n0 + 2 * c;
       if (ep.sumsq && j % 4 == 0) {   // a group starts only on a 32-column boundary (sumsq_group_cols % 32 == 0)
-        const int k = ep.sumsq_parts ? (n0 >> 7) : n0 / ep.sumsq_group_cols;
+        const int k = ep.sumsq_parts ? ((n0 + ep.sumsq_col0) >> 7) : (n0 + ep.sumsq_col0) / ep.sumsq_group_cols;
         if (k != key) {
           sumsq_flush(ep, rows[0], ok[0], lane, ss[0], key);
           sumsq_flush(ep, rows[1], ok[1], lane, ss[1], key);
@@ -320,7 +325,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     tma_prefetch_desc(&tmap_b);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init_a(full_bar(i), kE4M3 ? 1 + NUM_CONVERTERS / 32 : 1);   // e4m3: + one arrive per converter warp
-      mbar_init_a(empty_bar(i), 4);   // one arrive per warp of the consumer warpgroup that owns the stage's tile
+      mbar_init_a(empty_bar(i), 8);   // one arrive per consumer warp
     }
     for (int i = 0; i < W8_STAGES; ++i) {
       mbar_init_a(full8_bar(i), 1);
@@ -398,52 +403,38 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   } else {
     // ------------------------------- consumers ----------------------------------
     setmaxnreg_inc<CONSUMER_REGS>();
-    // Warpgroup cw takes the CTA's tiles 2 i + cw.  The ring holds the tiles' k-blocks in the producer's order, so each
-    // warpgroup steps over the other's num_kt stages after every tile of its own (and warpgroup 1 before its first).
+    // Both warpgroups share every tile: warpgroup cw takes rows [64 cw, 64 cw + 64) as one m64n256k16 per k16 step.
     const int cw = wg - 1;
     int stage = 0;
     uint32_t phase = 0;
-    auto skip_tile = [&]() {
-      const int s = stage + num_kt;
-      phase ^= (uint32_t)(s / STAGES) & 1u;
-      stage = s % STAGES;
-    };
-    if (cw == 1) skip_tile();
-    float acc[2][BN / 2];   // rows [0, 64) and [64, 128) of the tile
-    for (int tile = blockIdx.x + cw * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x) {
+    float acc[BN / 2];
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int m_blk, n_blk;
       tile_coords(tile, num_m, num_n, m_blk, n_blk);
-      // Ordering barrier (named barrier 1 + cw): a warpgroup starts waiting on the ring only after the other one has waited
-      // on every k-block before its tile, so no full-barrier wait runs more than one phase ahead (the parity would alias).
-      if (tile != (int)blockIdx.x) named_bar_sync(1 + cw);
       int prev = -1;
       for (int kb = 0; kb < num_kt; ++kb) {
         mbar_wait_a(full_bar(stage), phase);
         const uint32_t sa = sbase + stage * STAGE_BYTES;
-        const uint64_t da0 = wgmma_desc(sa, 16, 1024);
-        const uint64_t da1 = wgmma_desc(sa + 64 * 128, 16, 1024);
+        const uint64_t da = wgmma_desc(sa + cw * 64 * 128, 16, 1024);
         const uint64_t db = wgmma_desc(sa + A_STAGE_BYTES, 16, 1024);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {   // +32 B per K-step = +2 in the 16-byte address field
-          Wgmma<BN>::ss(acc[0], da0 + 2 * k, db + 2 * k, (kb | k) != 0);
-          Wgmma<BN>::ss(acc[1], da1 + 2 * k, db + 2 * k, (kb | k) != 0);
-        }
+        for (int k = 0; k < BK / 16; ++k)   // +32 B per K-step = +2 in the 16-byte address field
+          Wgmma<BN>::ss(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
         wgmma_commit();
         wgmma_wait<1>();   // the previous stage's MMAs have retired: its slot goes back to the producer
         if (prev >= 0 && lane == 0) mbar_arrive_a(empty_bar(prev));
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      if (tile + (int)gridDim.x < num_tiles) named_bar_arrive(2 - cw);   // the CTA's next tile is the other warpgroup's
       wgmma_wait<0>();
-      wgmma_fence_regs(acc[0]);
-      wgmma_fence_regs(acc[1]);
+      wgmma_fence_regs(acc);
       if (lane == 0) mbar_arrive_a(empty_bar(prev));
-      skip_tile();
-      const int row0 = m_blk * BM + (warp & 3) * 16;
-      epilogue<kAct, kF32, kFold>(ep, acc[0], M, N, row0, n_blk * BN, lane);
-      epilogue<kAct, kF32, kFold>(ep, acc[1], M, N, row0 + 64, n_blk * BN, lane);
+      const int row0 = m_blk * BM + cw * 64 + (warp & 3) * 16;
+#pragma unroll
+      for (int h = 0; h < BN / EPI_N; ++h)
+        epilogue<kAct, kF32, kFold>(ep, *reinterpret_cast<float(*)[EPI_N / 2]>(acc + h * EPI_N / 2), M, N, row0,
+                                    n_blk * BN + h * EPI_N, lane);
     }
   }
 }
@@ -505,6 +496,12 @@ int launch_kind(const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int 
   }
 }
 
+int make_w_tmap(CUtensorMap* tb, const void* W, int64_t ldw, int N, int K, bool e4m3) {
+  if (e4m3)   // the converters swizzle; the staging tile is plain 64-byte rows
+    return make_tmap_2d(tb, W, 1, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, BK, BN, /*swizzle_128b=*/false);
+  return make_tmap_2d(tb, W, 2, (uint64_t)K, (uint64_t)N, (uint64_t)ldw * 2, BK, BN);
+}
+
 // The arguments of one GEMM as both entry points take them: checked, then turned into the operand tensor maps and the
 // kernel's epilogue block.  `fn` names the entry point in the messages.
 int prepare(const char* fn, const void* A, int64_t lda, const void* W, int64_t ldw, int32_t M, int32_t N, int32_t K,
@@ -545,16 +542,13 @@ int prepare(const char* fn, const void* A, int64_t lda, const void* W, int64_t l
 
   int rc = make_tmap_2d(ta, A, 2, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, BK, BM);
   if (rc) return rc;
-  if (e->w_e4m3)   // the converters swizzle; the staging tile is plain 64-byte rows
-    rc = make_tmap_2d(tb, W, 1, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, BK, BN, /*swizzle_128b=*/false);
-  else
-    rc = make_tmap_2d(tb, W, 2, (uint64_t)K, (uint64_t)N, (uint64_t)ldw * 2, BK, BN);
+  rc = make_w_tmap(tb, W, ldw, N, K, e->w_e4m3 != 0);
   if (rc) return rc;
 
   ep->out = e->out; ep->ldo = e->ldo;
   ep->bias = e->bias; ep->gate = e->gate; ep->residual = e->residual; ep->ldr = e->ldr;
   ep->sumsq = e->sumsq; ep->sumsq_groups = e->sumsq_groups; ep->sumsq_group_cols = e->sumsq_group_cols;
-  ep->sumsq_parts = e->sumsq_parts;
+  ep->sumsq_parts = e->sumsq_parts; ep->sumsq_col0 = 0;
   ep->ln_stats = e->ln_stats; ep->ln_u = e->ln_u; ep->ln_inv_d = e->ln_dim > 0 ? 1.0f / (float)e->ln_dim : 0.f;
   ep->ln_eps = e->ln_eps;
   ep->a_next = reinterpret_cast<__nv_bfloat16*>(e->a_next); ep->ld_an = e->ld_an; ep->g_next = e->g_next;
@@ -590,7 +584,7 @@ extern "C" int svi_gemm_lora_bf16(const void* A, int64_t lda, const void* W, int
   if (rc) return rc;
   SVI_REQUIRE(lora && lora->U && lora->B, "svi_gemm_lora_bf16: null LoRA pointer");
   SVI_REQUIRE(lora->R > 0 && lora->R % BK == 0, "svi_gemm_lora_bf16: R must be a positive multiple of 64 (got %d)", lora->R);
-  SVI_REQUIRE(lora->group_cols == 0 || (lora->group_cols > 0 && lora->group_cols % BN == 0 && N % lora->group_cols == 0),
+  SVI_REQUIRE(lora->group_cols == 0 || (lora->group_cols > 0 && lora->group_cols % EPI_N == 0 && N % lora->group_cols == 0),
               "svi_gemm_lora_bf16: group_cols must be 0 or a multiple of 128 that divides N (got %d, N=%d)", lora->group_cols, N);
   const int64_t groups = lora->group_cols ? N / lora->group_cols : 1;
   SVI_REQUIRE((reinterpret_cast<uintptr_t>(lora->U) & 15) == 0 && (reinterpret_cast<uintptr_t>(lora->B) & 15) == 0,
@@ -601,15 +595,43 @@ extern "C" int svi_gemm_lora_bf16(const void* A, int64_t lda, const void* W, int
   SVI_REQUIRE(e->act == SVI_ACT_NONE || e->act == SVI_ACT_GELU_TANH,
               "svi_gemm_lora_bf16: activation %d has no LoRA kernel (none or GELU-tanh)", e->act);
   SVI_REQUIRE(!e->ln_stats && !e->a_next, "svi_gemm_lora_bf16: the LayerNorm fold (ln_* / a_next) cannot take a LoRA segment");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool f32 = e->out_is_f32 != 0;
   LoRAArgs<true> la;
   la.kb = lora->R / BK;
   la.group_cols = lora->group_cols;
-  rc = make_tmap_2d(&la.u, lora->U, 2, (uint64_t)(groups * lora->R), (uint64_t)M, (uint64_t)lora->ldu * 2, BK, BM);
-  if (rc) return rc;
-  rc = make_tmap_2d(&la.b, lora->B, 2, (uint64_t)lora->R, (uint64_t)N, (uint64_t)lora->ldb * 2, BK, BN);
-  if (rc) return rc;
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const bool f32 = e->out_is_f32 != 0;
-  return e->w_e4m3 ? launch_kind<true>(ta, tb, M, N, K, e->act, f32, false, ep, la, st)
-                   : launch_kind<false>(ta, tb, M, N, K, e->act, f32, false, ep, la, st);
+  if (lora->group_cols % BN == 0) {
+    rc = make_tmap_2d(&la.u, lora->U, 2, (uint64_t)(groups * lora->R), (uint64_t)M, (uint64_t)lora->ldu * 2, BK, BM);
+    if (rc) return rc;
+    rc = make_tmap_2d(&la.b, lora->B, 2, (uint64_t)lora->R, (uint64_t)N, (uint64_t)lora->ldb * 2, BK, BN);
+    if (rc) return rc;
+    return e->w_e4m3 ? launch_kind<true>(ta, tb, M, N, K, e->act, f32, false, ep, la, st)
+                     : launch_kind<false>(ta, tb, M, N, K, e->act, f32, false, ep, la, st);
+  }
+  // Groups of an odd multiple of 128 columns: a 256-column tile would straddle two groups, so each group is a launch of
+  // its own on its columns of W, B and the epilogue operands, with its block of U.
+  const int gc = lora->group_cols;
+  la.group_cols = 0;
+  for (int64_t g = 0; g < groups; ++g) {
+    const int64_t c0 = g * gc;
+    Epi eg = ep;
+    eg.out = static_cast<char*>(ep.out) + c0 * (f32 ? 4 : 2);
+    if (eg.bias) eg.bias += c0;
+    if (eg.gate) eg.gate += c0;
+    if (eg.residual) eg.residual += c0;
+    eg.sumsq_col0 = (int)c0;
+    CUtensorMap tw;
+    rc = make_w_tmap(&tw, static_cast<const char*>(W) + c0 * ldw * (e->w_e4m3 ? 1 : 2), ldw, gc, K, e->w_e4m3 != 0);
+    if (rc) return rc;
+    rc = make_tmap_2d(&la.u, static_cast<const char*>(lora->U) + g * lora->R * 2, 2, (uint64_t)lora->R, (uint64_t)M,
+                      (uint64_t)lora->ldu * 2, BK, BM);
+    if (rc) return rc;
+    rc = make_tmap_2d(&la.b, static_cast<const char*>(lora->B) + c0 * lora->ldb * 2, 2, (uint64_t)lora->R, (uint64_t)gc,
+                      (uint64_t)lora->ldb * 2, BK, BN);
+    if (rc) return rc;
+    rc = e->w_e4m3 ? launch_kind<true>(ta, tw, M, gc, K, e->act, f32, false, eg, la, st)
+                   : launch_kind<false>(ta, tw, M, gc, K, e->act, f32, false, eg, la, st);
+    if (rc) return rc;
+  }
+  return SVI_OK;
 }
