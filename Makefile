@@ -9,7 +9,7 @@ OBJS := $(patsubst $(CSRC)/%.cu,build/%.o,$(SRCS))
 
 all: $(LIB)
 
-build/%.o: $(CSRC)/%.cu $(CSRC)/common.cuh $(CSRC)/wgmma.cuh include/svi_b200.h include/svi_b200_lora.h include/svi_b200_rife.h include/svi_b200_esrgan.h include/svi_b200_fastblend.h include/svi_b200_unianimate.h include/svi_b200_replace.h include/svi_b200_quality.h include/svi_b200_reward.h
+build/%.o: $(CSRC)/%.cu $(CSRC)/common.cuh $(CSRC)/wgmma.cuh include/svi_b200.h include/svi_b200_lora.h include/svi_b200_rife.h include/svi_b200_esrgan.h include/svi_b200_fastblend.h include/svi_b200_fastblend_modes.h include/svi_b200_unianimate.h include/svi_b200_replace.h include/svi_b200_quality.h include/svi_b200_reward.h
 	@mkdir -p build
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> build/$*.ptxas.log || (cat build/$*.ptxas.log; exit 1)
 

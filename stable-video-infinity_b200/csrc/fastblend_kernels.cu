@@ -5,6 +5,7 @@
 // (oracle/fastblend_oracle.py) bit for bit.  Frames are channels-last, channel padded to 4.
 #include "common.cuh"
 #include "../../include/svi_b200_fastblend.h"
+#include "../../include/svi_b200_fastblend_modes.h"
 
 namespace svi {
 namespace fastblend {
@@ -337,5 +338,232 @@ extern "C" int svi_fastblend_table(const svi_fastblend_table_desc* d, void* stre
   }
   fastblend::table_kernel<<<fastblend::blocks(d->n_pix * 4, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(*d);
   SVI_CUDA_LAUNCH_CHECK("svi_fastblend_table");
+  return SVI_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// The balanced / accurate / interpolation modes (include/svi_b200_fastblend_modes.h).
+namespace svi {
+namespace fastblend {
+
+__global__ void candidate_kernel(svi_fastblend_candidate_desc d) {
+  const long long n = (long long)d.B * d.H * d.W;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int H = d.H, W = d.W;
+  const long long hw = (long long)H * W;
+  const int b = (int)(i / hw);
+  const long long pix = i - b * hw;
+  const int y = (int)(pix / W), x = (int)(pix % W);
+  const int2* nnf = reinterpret_cast<const int2*>(d.nnf_in);
+  const long long frame = b * hw;
+  int2 m;
+  if (d.mode == SVI_FASTBLEND_TRACK) {
+    int src;
+    if (d.pairwise) {
+      const int parity = b & 1, count = (d.B - parity + 1) / 2;
+      src = 2 * min(max(b / 2 + d.shift, 0), count - 1) + parity;
+    } else {
+      src = min(max(b + d.shift, 0), d.B - 1);
+    }
+    m = nnf[src * hw + pix];   // fields are inside the frame already: no clamp, as the reference's track_step
+  } else if (d.mode == SVI_FASTBLEND_NEIGHBOUR) {
+    switch (d.dir) {
+      case 0: m = nnf[frame + (long long)max(y - 1, 0) * W + x]; m.x += 1; break;
+      case 1: m = nnf[frame + (long long)y * W + max(x - 1, 0)]; m.y += 1; break;
+      case 2: m = nnf[frame + (long long)min(y + 1, H - 1) * W + x]; m.x -= 1; break;
+      default: m = nnf[frame + (long long)y * W + min(x + 1, W - 1)]; m.y -= 1; break;
+    }
+    m = make_int2(min(max(m.x, 0), H - 1), min(max(m.y, 0), W - 1));
+  } else {
+    const uint32_t span = (uint32_t)(2 * d.radius + 1);
+    const uint32_t e0 = (uint32_t)(i * 2);
+    m = nnf[i];
+    m.x += -d.radius + (int)(stream_u(d.draw, e0) % span);
+    m.y += -d.radius + (int)(stream_u(d.draw, e0 + 1) % span);
+    m = make_int2(min(max(m.x, 0), H - 1), min(max(m.y, 0), W - 1));
+  }
+  reinterpret_cast<int2*>(d.nnf_out)[i] = m;
+}
+
+// The error of a given candidate and the select.  The block layout is the step kernel's: a 16 x 16 tile of one frame,
+// its target guide window (and target style window, unless pairwise) with an r-pixel halo in shared memory.
+__global__ void __launch_bounds__(kTile * kTile) select_kernel(svi_fastblend_select_desc d) {
+  extern __shared__ float4 win[];
+  const int H = d.H, W = d.W, r = (d.patch_size - 1) / 2, side = kTile + 2 * r;
+  float4* tg = win;
+  float4* ts = win + side * side;
+  const int b = blockIdx.z, y0 = blockIdx.y * kTile, x0 = blockIdx.x * kTile;
+  const long long hw = (long long)H * W, frame = (long long)b * hw;
+  const float4* tgt_guide = reinterpret_cast<const float4*>(d.tgt_guide) + frame;
+  const float4* tgt_style = d.pairwise ? nullptr : reinterpret_cast<const float4*>(d.tgt_style) + (d.style_shared ? 0 : frame);
+  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int j = threadIdx.y * kTile + threadIdx.x; j < side * side; j += kTile * kTile) {
+    const int wy = y0 - r + j / side, wx = x0 - r + j % side;
+    const bool in = wy >= 0 && wy < H && wx >= 0 && wx < W;
+    tg[j] = in ? __ldg(tgt_guide + (long long)wy * W + wx) : zero;
+    if (tgt_style) ts[j] = in ? __ldg(tgt_style + (long long)wy * W + wx) : zero;
+  }
+  __syncthreads();
+  const int y = y0 + threadIdx.y, x = x0 + threadIdx.x;
+  if (y >= H || x >= W) return;
+  const long long pix = (long long)y * W + x, o = frame + pix;
+  const int2* cand = reinterpret_cast<const int2*>(d.cand);
+  const int2 c = cand[o];
+  const float4* sg = reinterpret_cast<const float4*>(d.src_guide) + frame;
+  float eg = 0.f, es = 0.f;
+  if (!d.pairwise) {
+    const float4* ss = reinterpret_cast<const float4*>(d.src_style) + frame;
+    for (int px = -r; px <= r; px++) {
+      const int sy = c.x + px;
+      const bool row_in = sy >= 0 && sy < H;
+      const float4* tg_row = tg + (threadIdx.y + r + px) * side + threadIdx.x + r;
+      const float4* ts_row = ts + (threadIdx.y + r + px) * side + threadIdx.x + r;
+      for (int py = -r; py <= r; py++) {
+        const int sx = c.y + py;
+        const bool in = row_in && sx >= 0 && sx < W;
+        const long long s = (long long)sy * W + sx;
+        eg = sq_acc(eg, tg_row[py], in ? __ldg(sg + s) : zero);
+        es = sq_acc(es, ts_row[py], in ? __ldg(ss + s) : zero);
+      }
+    }
+  } else {
+    // both members of pair k evaluate the pair's style term in the same order, so they hold the same bits
+    const long long fa = (long long)(b & ~1) * hw, fb = fa + hw;
+    const int2 ca = cand[fa + pix], cb = cand[fb + pix];
+    const float4* sa = reinterpret_cast<const float4*>(d.src_style) + fa;
+    const float4* sb = reinterpret_cast<const float4*>(d.src_style) + fb;
+    for (int px = -r; px <= r; px++) {
+      const int sy = c.x + px, ay = ca.x + px, by = cb.x + px;
+      const float4* tg_row = tg + (threadIdx.y + r + px) * side + threadIdx.x + r;
+      for (int py = -r; py <= r; py++) {
+        const int sx = c.y + py, ax = ca.y + py, bx = cb.y + py;
+        const bool in = sy >= 0 && sy < H && sx >= 0 && sx < W;
+        const bool in_a = ay >= 0 && ay < H && ax >= 0 && ax < W;
+        const bool in_b = by >= 0 && by < H && bx >= 0 && bx < W;
+        eg = sq_acc(eg, tg_row[py], in ? __ldg(sg + (long long)sy * W + sx) : zero);
+        es = sq_acc(es, in_a ? __ldg(sa + (long long)ay * W + ax) : zero, in_b ? __ldg(sb + (long long)by * W + bx) : zero);
+      }
+    }
+  }
+  const float e = __fadd_rn(__fmul_rn(eg, d.guide_weight), es);
+  int2* nnf_out = reinterpret_cast<int2*>(d.nnf_out);
+  if (!d.select || e < d.err_in[o]) {
+    nnf_out[o] = c;
+    d.err_out[o] = e;
+  } else {
+    nnf_out[o] = reinterpret_cast<const int2*>(d.nnf_in)[o];
+    d.err_out[o] = d.err_in[o];
+  }
+}
+
+__global__ void batch_mean_kernel(const float* __restrict__ src, int B, long long n, float* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n * 4) return;
+  if ((i & 3) == 3) { out[i] = 0.f; return; }
+  float s = src[i];
+  for (int b = 1; b < B; b++) s = __fadd_rn(s, src[(long long)b * n * 4 + i]);
+  out[i] = __fdiv_rn(s, (float)B);
+}
+
+__global__ void running_mean_kernel(const void* frame, int frame_type, double s, const float* __restrict__ result,
+                                    float divisor, long long n, double* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n * 4) return;
+  if ((i & 3) == 3) { out[i] = 0.0; return; }
+  const double f = frame_type == SVI_FASTBLEND_F64 ? static_cast<const double*>(frame)[i]
+                                                   : (double)static_cast<const float*>(frame)[i];
+  out[i] = __dadd_rn(__dmul_rn(f, s), (double)__fdiv_rn(result[i], divisor));
+}
+
+__global__ void to_u8_kernel(const void* a, int a_type, long long n, uint8_t* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n * 3) return;
+  const long long e = (i / 3) * 4 + i % 3;
+  const double v = a_type == SVI_FASTBLEND_F64 ? static_cast<const double*>(a)[e] : (double)static_cast<const float*>(a)[e];
+  out[i] = (uint8_t)(int)fmin(fmax(v, 0.0), 255.0);
+}
+
+}  // namespace fastblend
+}  // namespace svi
+
+extern "C" int svi_fastblend_candidate(const svi_fastblend_candidate_desc* d, void* stream) {
+  SVI_REQUIRE(d && d->nnf_in && d->nnf_out && d->nnf_in != d->nnf_out, "svi_fastblend_candidate: null or aliased field");
+  SVI_REQUIRE(d->B > 0 && d->H > 0 && d->W > 0, "svi_fastblend_candidate: bad shape");
+  SVI_REQUIRE((long long)d->B * d->H * d->W * 2 < (1LL << 32), "svi_fastblend_candidate: batch too large for the stream index");
+  SVI_REQUIRE(d->mode == SVI_FASTBLEND_NEIGHBOUR || d->mode == SVI_FASTBLEND_RANDOM || d->mode == SVI_FASTBLEND_TRACK,
+              "svi_fastblend_candidate: unknown mode");
+  SVI_REQUIRE(d->mode != SVI_FASTBLEND_NEIGHBOUR || (d->dir >= 0 && d->dir <= 3), "svi_fastblend_candidate: dir must be 0..3");
+  SVI_REQUIRE(d->mode != SVI_FASTBLEND_RANDOM || (d->radius >= 0 && d->radius < (1 << 20)), "svi_fastblend_candidate: bad radius");
+  SVI_REQUIRE(d->mode != SVI_FASTBLEND_TRACK || (d->shift != 0 && (!d->pairwise || d->B % 2 == 0)),
+              "svi_fastblend_candidate: tracking needs a nonzero shift (and an even batch when pairwise)");
+  SVI_REQUIRE(((reinterpret_cast<uintptr_t>(d->nnf_in) | reinterpret_cast<uintptr_t>(d->nnf_out)) & 7) == 0,
+              "svi_fastblend_candidate: fields must be 8-byte aligned");
+  fastblend::candidate_kernel<<<fastblend::blocks((long long)d->B * d->H * d->W, 256), 256, 0,
+                                static_cast<cudaStream_t>(stream)>>>(*d);
+  SVI_CUDA_LAUNCH_CHECK("svi_fastblend_candidate");
+  return SVI_OK;
+}
+
+extern "C" int svi_fastblend_select(const svi_fastblend_select_desc* d, void* stream) {
+  SVI_REQUIRE(d, "svi_fastblend_select: null descriptor");
+  SVI_REQUIRE(d->src_guide && d->src_style && d->tgt_guide && d->cand && d->nnf_out && d->err_out &&
+                  (d->pairwise || d->tgt_style) && (!d->select || (d->nnf_in && d->err_in)),
+              "svi_fastblend_select: null pointer");
+  SVI_REQUIRE(d->B > 0 && d->H > 0 && d->W > 0 && d->B <= 65535, "svi_fastblend_select: bad shape");
+  SVI_REQUIRE(d->patch_size >= 1 && d->patch_size <= SVI_FASTBLEND_MAX_PATCH, "svi_fastblend_select: patch size out of range");
+  SVI_REQUIRE((d->select == 0 || d->select == 1) && (d->style_shared == 0 || d->style_shared == 1) &&
+                  (d->pairwise == 0 || d->pairwise == 1),
+              "svi_fastblend_select: select, style_shared and pairwise are 0 or 1");
+  SVI_REQUIRE(!d->pairwise || d->B % 2 == 0, "svi_fastblend_select: the pairwise error needs an even batch");
+  SVI_REQUIRE((const void*)d->nnf_out != (const void*)d->cand && (const void*)d->nnf_out != (const void*)d->nnf_in &&
+                  (const void*)d->err_out != (const void*)d->err_in,
+              "svi_fastblend_select: outputs must not alias inputs");
+  const uintptr_t f = reinterpret_cast<uintptr_t>(d->src_guide) | reinterpret_cast<uintptr_t>(d->src_style) |
+                      reinterpret_cast<uintptr_t>(d->tgt_guide) | reinterpret_cast<uintptr_t>(d->tgt_style);
+  const uintptr_t n = reinterpret_cast<uintptr_t>(d->cand) | reinterpret_cast<uintptr_t>(d->nnf_in) |
+                      reinterpret_cast<uintptr_t>(d->nnf_out);
+  SVI_REQUIRE((f & 15) == 0 && (n & 7) == 0, "svi_fastblend_select: frames must be 16-byte and fields 8-byte aligned");
+  const int r = (d->patch_size - 1) / 2, side = fastblend::kTile + 2 * r;
+  const size_t smem = (size_t)2 * side * side * sizeof(float4);
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(fastblend::select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    SVI_REQUIRE(e == cudaSuccess, "svi_fastblend_select: cannot reserve %zu bytes of shared memory", smem);
+  }
+  const dim3 grid((d->W + fastblend::kTile - 1) / fastblend::kTile, (d->H + fastblend::kTile - 1) / fastblend::kTile, d->B);
+  fastblend::select_kernel<<<grid, dim3(fastblend::kTile, fastblend::kTile), smem, static_cast<cudaStream_t>(stream)>>>(*d);
+  SVI_CUDA_LAUNCH_CHECK("svi_fastblend_select");
+  return SVI_OK;
+}
+
+extern "C" int svi_fastblend_batch_mean(const float* src, int32_t B, int64_t n_pix, float* out, void* stream) {
+  SVI_REQUIRE(src && out && (const void*)src != (const void*)out, "svi_fastblend_batch_mean: null or aliased pointer");
+  SVI_REQUIRE(B > 0 && n_pix > 0 && n_pix < (1LL << 40), "svi_fastblend_batch_mean: bad shape");
+  fastblend::batch_mean_kernel<<<fastblend::blocks(n_pix * 4, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      src, B, (long long)n_pix, out);
+  SVI_CUDA_LAUNCH_CHECK("svi_fastblend_batch_mean");
+  return SVI_OK;
+}
+
+extern "C" int svi_fastblend_running_mean(const void* frame, int32_t frame_type, double s, const float* result,
+                                          float divisor, int64_t n_pix, double* out, void* stream) {
+  SVI_REQUIRE(frame && result && out, "svi_fastblend_running_mean: null pointer");
+  SVI_REQUIRE(frame_type == SVI_FASTBLEND_U8 || frame_type == SVI_FASTBLEND_F64,
+              "svi_fastblend_running_mean: the frame is uint8 (held as f32) or f64");
+  SVI_REQUIRE(n_pix > 0 && n_pix < (1LL << 40), "svi_fastblend_running_mean: bad pixel count");
+  fastblend::running_mean_kernel<<<fastblend::blocks(n_pix * 4, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      frame, frame_type, s, result, divisor, (long long)n_pix, out);
+  SVI_CUDA_LAUNCH_CHECK("svi_fastblend_running_mean");
+  return SVI_OK;
+}
+
+extern "C" int svi_fastblend_to_u8(const void* a, int32_t a_type, int64_t n_pix, uint8_t* out, void* stream) {
+  SVI_REQUIRE(a && out, "svi_fastblend_to_u8: null pointer");
+  SVI_REQUIRE(a_type == SVI_FASTBLEND_U8 || a_type == SVI_FASTBLEND_F32 || a_type == SVI_FASTBLEND_F64,
+              "svi_fastblend_to_u8: bad operand type");
+  SVI_REQUIRE(n_pix > 0 && n_pix < (1LL << 40), "svi_fastblend_to_u8: bad pixel count");
+  fastblend::to_u8_kernel<<<fastblend::blocks(n_pix * 3, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      a, a_type, (long long)n_pix, out);
+  SVI_CUDA_LAUNCH_CHECK("svi_fastblend_to_u8");
   return SVI_OK;
 }

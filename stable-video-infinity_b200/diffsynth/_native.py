@@ -1,6 +1,7 @@
 """ctypes binding of the C-ABI kernel library ``libsvi_b200.so`` (declared in ``include/svi_b200.h``,
 ``include/svi_b200_lora.h``, ``include/svi_b200_rife.h``, ``include/svi_b200_esrgan.h``,
-``include/svi_b200_fastblend.h``, ``include/svi_b200_unianimate.h``, ``include/svi_b200_replace.h``,
+``include/svi_b200_fastblend.h``, ``include/svi_b200_fastblend_modes.h``,
+``include/svi_b200_unianimate.h``, ``include/svi_b200_replace.h``,
 ``include/svi_b200_quality.h`` and ``include/svi_b200_reward.h``).
 
 This is the only door between the Python host code and the hand-written sm_90a kernels.  There is no
@@ -218,6 +219,35 @@ FB_CURRENT, FB_NEIGHBOUR, FB_RANDOM = 0, 1, 2
 FB_U8, FB_F32, FB_F64 = 0, 1, 2
 FB_MEAN, FB_HALF, FB_WSUM = 0, 1, 2
 
+
+class FastblendCandidateDesc(_c.Structure):
+    """Mirror of ``svi_fastblend_candidate_desc`` (include/svi_b200_fastblend_modes.h)."""
+    _fields_ = [
+        ("nnf_in", _vp), ("nnf_out", _vp), ("B", _i32), ("H", _i32), ("W", _i32), ("mode", _i32), ("dir", _i32),
+        ("draw", _c.c_uint32), ("radius", _i32), ("shift", _i32), ("pairwise", _i32),
+    ]
+
+
+class FastblendSelectDesc(_c.Structure):
+    """Mirror of ``svi_fastblend_select_desc`` (include/svi_b200_fastblend_modes.h)."""
+    _fields_ = [
+        ("src_guide", _vp), ("src_style", _vp), ("tgt_guide", _vp), ("tgt_style", _vp), ("cand", _vp),
+        ("nnf_in", _vp), ("err_in", _vp), ("nnf_out", _vp), ("err_out", _vp),
+        ("B", _i32), ("H", _i32), ("W", _i32), ("patch_size", _i32), ("select", _i32), ("style_shared", _i32),
+        ("pairwise", _i32), ("guide_weight", _f32),
+    ]
+
+
+# the same for include/svi_b200_fastblend_modes.h (the balanced / accurate / interpolation modes)
+FASTBLEND_MODES_SIGNATURES = {
+    "svi_fastblend_candidate": (_i32, [_c.POINTER(FastblendCandidateDesc), _vp]),
+    "svi_fastblend_select": (_i32, [_c.POINTER(FastblendSelectDesc), _vp]),
+    "svi_fastblend_batch_mean": (_i32, [_vp, _i32, _i64, _vp, _vp]),
+    "svi_fastblend_running_mean": (_i32, [_vp, _i32, _c.c_double, _vp, _f32, _i64, _vp, _vp]),
+    "svi_fastblend_to_u8": (_i32, [_vp, _i32, _i64, _vp, _vp]),
+}
+FB_TRACK = 3
+
 # the same for include/svi_b200_unianimate.h
 UNIANIMATE_SIGNATURES = {
     "svi_window_accumulate": (_i32, [_vp, _i32, _i32, _i64, _i32, _vp, _i32, _i32, _vp]),
@@ -272,7 +302,7 @@ def load():
             f"`python -c 'import __graft_entry__ as g; g.build()'` (or `make`) — there is no CPU fallback.")
     lib = ctypes.CDLL(_LIB_PATH)
     for name, (res, args) in (SIGNATURES | LORA_SIGNATURES | RIFE_SIGNATURES | ESRGAN_SIGNATURES |
-                        FASTBLEND_SIGNATURES | UNIANIMATE_SIGNATURES | REPLACE_SIGNATURES | QUALITY_SIGNATURES |
+                        FASTBLEND_SIGNATURES | FASTBLEND_MODES_SIGNATURES | UNIANIMATE_SIGNATURES | REPLACE_SIGNATURES | QUALITY_SIGNATURES |
                         REWARD_SIGNATURES).items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing: fail loudly
         fn.restype = res
@@ -1132,6 +1162,83 @@ def fastblend_table(op, out, a, sa=0.0, b=None, sb=0.0, c=None, sc=0.0, a_u8=Fal
     else:
         d.out, d.out_type = operand(out, False, "out")
     _check(load().svi_fastblend_table(ctypes.byref(d), _stream()), "svi_fastblend_table")
+    return out
+
+
+# --------------------------------------------------------------------------------------------- FastBlend modes (include/svi_b200_fastblend_modes.h)
+def fastblend_candidate(nnf_in, nnf_out, mode, dir=0, draw=0, radius=0, shift=0, pairwise=False):
+    """nnf_out int32 [B, H, W, 2] = the candidate field of nnf_in (svi_fastblend_candidate): a neighbour, random or
+    tracking step."""
+    B, H, W, _ = nnf_in.shape
+    if nnf_out.shape != nnf_in.shape:
+        raise RuntimeError("svi_b200.fastblend_candidate: nnf_in and nnf_out must be [B, H, W, 2] of one shape")
+    d = FastblendCandidateDesc()
+    d.nnf_in, d.nnf_out = _fb_frames(nnf_in, "nnf_in", torch.int32, 2), _fb_frames(nnf_out, "nnf_out", torch.int32, 2)
+    d.B, d.H, d.W, d.mode, d.dir = B, H, W, int(mode), int(dir)
+    d.draw, d.radius, d.shift, d.pairwise = int(draw) & 0xFFFFFFFF, int(radius), int(shift), int(bool(pairwise))
+    _check(load().svi_fastblend_candidate(ctypes.byref(d), _stream()), "svi_fastblend_candidate")
+    return nnf_out
+
+
+def fastblend_select(src_guide, src_style, tgt_guide, tgt_style, cand, nnf_in, err_in, nnf_out, err_out, patch_size,
+                     guide_weight, pairwise=False):
+    """The error of the candidate field `cand` and the select (svi_fastblend_select).  frames f32 [B, H, W, 4]; tgt_style
+    is [B, H, W, 4], one [H, W, 4] frame shared by every entry, or None with the pairwise error; nnf_in / err_in None
+    write the candidate and its error unconditionally."""
+    B, H, W, _ = src_guide.shape
+    if any(t.shape != src_guide.shape for t in (src_style, tgt_guide)) or tuple(cand.shape) != (B, H, W, 2) \
+            or nnf_out.shape != cand.shape or tuple(err_out.shape) != (B, H, W) \
+            or (nnf_in is not None and nnf_in.shape != cand.shape) or (err_in is not None and err_in.shape != err_out.shape) \
+            or (nnf_in is None) != (err_in is None):
+        raise RuntimeError("svi_b200.fastblend_select: frames, fields and errors must describe the same [B, H, W] pixels")
+    d = FastblendSelectDesc()
+    d.src_guide, d.src_style = _fb_frames(src_guide, "src_guide"), _fb_frames(src_style, "src_style")
+    d.tgt_guide = _fb_frames(tgt_guide, "tgt_guide")
+    if tgt_style is not None:
+        shared = tgt_style.dim() == 3
+        if tuple(tgt_style.shape) != ((H, W, 4) if shared else (B, H, W, 4)) or not tgt_style.is_contiguous():
+            raise RuntimeError("svi_b200.fastblend_select: tgt_style must be contiguous [B, H, W, 4] or [H, W, 4]")
+        d.tgt_style, d.style_shared = _ptr(tgt_style, torch.float32, "tgt_style"), int(shared)
+    d.cand = _fb_frames(cand, "cand", torch.int32, 2)
+    d.nnf_in = None if nnf_in is None else _fb_frames(nnf_in, "nnf_in", torch.int32, 2)
+    d.err_in, d.err_out = _contig(err_in, torch.float32, "err_in"), _contig(err_out, torch.float32, "err_out")
+    d.nnf_out = _fb_frames(nnf_out, "nnf_out", torch.int32, 2)
+    d.B, d.H, d.W, d.patch_size = B, H, W, int(patch_size)
+    d.select, d.pairwise, d.guide_weight = int(nnf_in is not None), int(bool(pairwise)), float(guide_weight)
+    _check(load().svi_fastblend_select(ctypes.byref(d), _stream()), "svi_fastblend_select")
+
+
+def fastblend_batch_mean(src, out):
+    """out f32 [H, W, 4] = the f32 mean over B of src f32 [B, H, W, 4], summed in b order (svi_fastblend_batch_mean)."""
+    B = src.shape[0]
+    if tuple(out.shape) != tuple(src.shape[1:]) or src.shape[-1] != 4:
+        raise RuntimeError("svi_b200.fastblend_batch_mean: src must be [B, ..., 4] and out one entry of it")
+    _check(load().svi_fastblend_batch_mean(_contig(src, torch.float32, "src"), B, out.numel() // 4,
+                                           _contig(out, torch.float32, "out"), _stream()), "svi_fastblend_batch_mean")
+    return out
+
+
+def fastblend_running_mean(frame, s, result, divisor, out, frame_u8=False):
+    """out f64 [..., 4] = f64(frame) * s + f64(result / f32(divisor)) (svi_fastblend_running_mean); frame is f64, or with
+    frame_u8 a uint8 frame held as its f32 values; result f32."""
+    n = out.numel() // 4
+    if out.dtype != torch.float64 or out.shape[-1] != 4 or frame.numel() != out.numel() or result.numel() != out.numel():
+        raise RuntimeError("svi_b200.fastblend_running_mean: frame, result and out must be [..., 4] of one pixel count")
+    ftype = FB_U8 if frame_u8 else FB_F64
+    _check(load().svi_fastblend_running_mean(_contig(frame, torch.float32 if frame_u8 else torch.float64, "frame"), ftype,
+                                             float(s), _contig(result, torch.float32, "result"), float(divisor), n,
+                                             _contig(out, torch.float64, "out"), _stream()), "svi_fastblend_running_mean")
+    return out
+
+
+def fastblend_to_u8(a, out, a_u8=False):
+    """out uint8 [..., 3] = a f32 / f64 [..., 4] clipped to [0, 255] and truncated (svi_fastblend_to_u8)."""
+    n = a.numel() // 4
+    if a.shape[-1] != 4 or out.shape[-1] != 3 or out.numel() // 3 != n or a.dtype not in _FB_TYPES:
+        raise RuntimeError("svi_b200.fastblend_to_u8: a must be f32 / f64 [..., 4] and out uint8 [..., 3] of as many pixels")
+    atype = FB_U8 if a_u8 else _FB_TYPES[a.dtype]
+    _check(load().svi_fastblend_to_u8(_contig(a, a.dtype, "a"), atype, n, _contig(out, torch.uint8, "out"), _stream()),
+           "svi_fastblend_to_u8")
     return out
 
 

@@ -1,9 +1,11 @@
-"""FastBlend video deflickering on the native sm_90a kernels (include/svi_b200_fastblend.h).
+"""FastBlend video deflickering on the native sm_90a kernels (include/svi_b200_fastblend.h and
+include/svi_b200_fastblend_modes.h).
 
 The reference's names and call semantics (diffsynth/extensions/FastBlend: __init__.py, runners/fast.py,
 patch_match.py): `FastBlendSmoother()(frames)` matches every frame against the frames of a window around it with a
 coarse-to-fine PatchMatch (`PyramidPatchMatcher`), remaps them onto it and blends them through the tree tables of
 `TableManager`.  The whole computation runs on the device; frames cross the bus once as bytes in each direction.
+The balanced and accurate modes and keyframe interpolation are the runners of `.runners`.
 
 Exactness: every kernel repeats the reference's arithmetic in its order, each operation rounded on its own, and the host
 keeps the reference's task order and batching (batch composition changes results: PyramidPatchMatcher's NNF upscale adds
@@ -41,17 +43,17 @@ def _unsupported(option, value, why):
 
 class PyramidPatchMatcher:
     """Coarse-to-fine PatchMatch of target frames against source frames (patch_match.py:205).  `gpu_id` selects the
-    device; `threads_per_block` is accepted and has no effect (the kernels choose their own launch shape)."""
+    device; `threads_per_block` is accepted and has no effect (the kernels choose their own launch shape).
+
+    `use_mean_target_style` measures every candidate's style error against the batch mean of the source style remapped
+    through that candidate; `use_pairwise_patch_error` gives entries 2k and 2k + 1 one shared style error, the patch
+    distance between their source styles (the batch must be even); `tracking_window_size` T adds 2T steps per
+    iteration whose candidates are the fields of the batch entries d = 1, -1, ..., T, -T away (within each parity class
+    with the pairwise error)."""
 
     def __init__(self, image_height, image_width, channel, minimum_patch_size, threads_per_block=8, num_iter=5, gpu_id=0,
                  guide_weight=10.0, use_mean_target_style=False, use_pairwise_patch_error=False, tracking_window_size=0,
                  initialize="identity"):
-        if use_mean_target_style:
-            raise _unsupported("use_mean_target_style", use_mean_target_style, "only the fast mode's per-frame target style")
-        if use_pairwise_patch_error:
-            raise _unsupported("use_pairwise_patch_error", use_pairwise_patch_error, "only the fast mode's patch error")
-        if tracking_window_size > 0:
-            raise _unsupported("tracking_window_size", tracking_window_size, "tracking steps are not implemented")
         if initialize != "identity":
             raise _unsupported("initialize", initialize, "only the identity initialisation is implemented")
         if channel != 3:
@@ -70,6 +72,8 @@ class PyramidPatchMatcher:
         self.patch_size_list = [minimum_patch_size + i * 2 for i in range(num_iter)][::-1]
         self.minimum_patch_size, self.num_iter = minimum_patch_size, num_iter
         self.gpu_id, self.guide_weight, self.initialize = gpu_id, guide_weight, initialize
+        self.use_mean_target_style, self.use_pairwise_patch_error = bool(use_mean_target_style), bool(use_pairwise_patch_error)
+        self.tracking_window_size = int(tracking_window_size)
         self.device = _device(gpu_id)
         self.draws = 0        # the random stream's counter: one per randint / permutation the reference would draw
 
@@ -94,6 +98,8 @@ class PyramidPatchMatcher:
         """f32 [B, H, W, 4] frames on the device -> (nnf int32 [B, H, W, 2], target_style f32 [B, H, W, 4])."""
         B = source_guide.shape[0]
         self.check_batch(B)
+        if self.use_pairwise_patch_error and B % 2:
+            raise ValueError(f"FastBlend: the pairwise patch error pairs entries 2k and 2k + 1; a batch of {B} is odd")
         nv.require_cuda(self.device, "FastBlend")
         nnf = ts = None
         for level, (h, w) in enumerate(zip(self.pyramid_heights, self.pyramid_widths)):
@@ -150,12 +156,20 @@ class PyramidPatchMatcher:
 
     def _level(self, sg, tg, ss, nnf):
         """one level's PatchMatch (patch_match.py:191-202): per iteration the remapped style, the error of the current
-        field, four neighbour steps in a drawn order and three random steps; each step reads one field / error pair and
-        writes the other."""
+        field, four neighbour steps in a drawn order, three random steps and 2T tracking steps; each step reads one
+        field / error pair and writes the other.  Without the mean or pairwise error a neighbour or random step is one
+        svi_fastblend_step; otherwise, and for tracking, the candidate field is built first and then evaluated
+        (svi_fastblend_candidate, then svi_fastblend_select), the mean target style remapped and averaged in between."""
         B, H, W, _ = sg.shape
+        plain = not (self.use_mean_target_style or self.use_pairwise_patch_error)
+        pairwise = self.use_pairwise_patch_error
+        mean_style = self.use_mean_target_style and not pairwise     # with both, the reference's mean goes unused
         ts = torch.empty_like(ss)
         fields = [nnf, torch.empty_like(nnf)]
         errs = [torch.empty(B, H, W, dtype=torch.float32, device=self.device) for _ in range(2)]
+        cand = torch.empty_like(nnf) if not plain or self.tracking_window_size > 0 else None
+        remapped = torch.empty_like(ss) if mean_style else None
+        mean = torch.empty(H, W, 4, dtype=torch.float32, device=self.device) if mean_style else None
         cur = 0
 
         def step(mode, patch, **kw):
@@ -164,14 +178,39 @@ class PyramidPatchMatcher:
                               errs[1 - cur], patch, mode, self.guide_weight, **kw)
             cur = 1 - cur
 
+        def select(candidate, patch, first=False):
+            nonlocal cur
+            target = ts
+            if pairwise:
+                target = None
+            elif mean_style:                                      # get_error (patch_match.py:76-87)
+                nv.fastblend_remap(ss, candidate, patch, remapped)
+                target = nv.fastblend_batch_mean(remapped, mean)
+            nv.fastblend_select(sg, ss, tg, target, candidate, None if first else fields[cur], None if first else errs[cur],
+                                fields[1 - cur], errs[1 - cur], patch, self.guide_weight, pairwise=pairwise)
+            cur = 1 - cur
+
+        def propose(mode, patch, **kw):
+            if plain and mode != nv.FB_TRACK:
+                step(mode, patch, **kw)
+            else:
+                nv.fastblend_candidate(fields[cur], cand, mode, pairwise=pairwise, **kw)
+                select(cand, patch)
+
         for patch in self.patch_size_list:
-            nv.fastblend_remap(ss, fields[cur], patch, ts)
-            step(nv.FB_CURRENT, patch)
+            if plain:
+                nv.fastblend_remap(ss, fields[cur], patch, ts)
+                step(nv.FB_CURRENT, patch)
+            else:
+                select(fields[cur], patch, first=True)
             perm = self._permutation4()
             for d in perm:
-                step(nv.FB_NEIGHBOUR, patch, dir=d)
+                propose(nv.FB_NEIGHBOUR, patch, dir=d)
             for _ in range(RANDOM_SEARCH_STEPS):
-                step(nv.FB_RANDOM, patch, draw=self._draw(), radius=RANDOM_SEARCH_RANGE)
+                propose(nv.FB_RANDOM, patch, draw=self._draw(), radius=RANDOM_SEARCH_RANGE)
+            for d in range(1, self.tracking_window_size + 1):          # track (patch_match.py:177-183)
+                propose(nv.FB_TRACK, patch, shift=d)
+                propose(nv.FB_TRACK, patch, shift=-d)
         out = torch.empty_like(ss)
         nv.fastblend_remap(ss, fields[cur], self.patch_size_list[-1], out)
         return fields[cur], out
@@ -304,6 +343,42 @@ def stage_frames(frames, device):
     return [Frame(f, "uint8") for f in staged]
 
 
+def stage_pair(frames_guide, frames_style, device):
+    """stage_frames of the guide and style frames (the guide is the style when they are the same object); both of one
+    size and count"""
+    style = stage_frames(frames_style, device)
+    guide = style if frames_guide is frames_style else stage_frames(frames_guide, device)
+    if len(guide) != len(style) or guide[0].data.shape != style[0].data.shape:
+        raise ValueError("FastBlend: original and rendered frames must be as many and of one size")
+    return guide, style
+
+
+def frame_size(frame):
+    """(H, W) of a PIL image or [H, W, 3] array"""
+    return np.asarray(frame.convert("RGB") if isinstance(frame, Image.Image) else frame).shape[:2]
+
+
+def fast_mode(frames_guide, frames_style, batch_size, window_size, ebsynth_config):
+    """The fast mode (runners/fast.py, __init__.py): the left and right tree tables and their merge.  Frames (PIL images
+    or uint8 [H, W, 3] arrays) -> PIL images."""
+    H, W = frame_size(frames_style[0])
+    engine = PyramidPatchMatcher(image_height=H, image_width=W, channel=3, **ebsynth_config)
+    nv.require_cuda(engine.device, "FastBlend")
+    guide, style = stage_pair(frames_guide, frames_style, engine.device)
+    tm = TableManager()
+    table_l = tm.build_remapping_table(guide, style, engine, batch_size)
+    table_l = tm.process_window_sum(guide, tm.remapping_table_to_blending_table(table_l), engine, window_size, batch_size)
+    table_r = tm.build_remapping_table(guide[::-1], style[::-1], engine, batch_size)
+    table_r = tm.process_window_sum(guide[::-1], tm.remapping_table_to_blending_table(table_r), engine, window_size,
+                                    batch_size)[::-1]
+    out = torch.empty(len(style), H, W, 3, dtype=torch.uint8, device=engine.device)
+    for i, ((fl, wl), fm, (fr, wr)) in enumerate(zip(table_l, style, table_r)):
+        w = wl - 1 + wr                                         # the reference's weight_m = -1
+        nv.fastblend_table(nv.FB_WSUM, out[i], fl.data, wl / w, fm.data, -1 / w, c=fr.data, sc=wr / w,
+                           a_u8=fl.kind == "uint8", b_u8=True, c_u8=fr.kind == "uint8")
+    return [Image.fromarray(f) for f in out.cpu().numpy()]
+
+
 class FastBlendSmoother:
     """FastBlend's fast mode (__init__.py:7): deflickers rendered frames, guided by the original frames or, with
     original_frames=None, by the rendered frames themselves."""
@@ -326,27 +401,15 @@ class FastBlendSmoother:
         return FastBlendSmoother()
 
     def run(self, frames_guide, frames_style, batch_size, window_size, ebsynth_config):
-        """Frames (PIL images or uint8 [H, W, 3] arrays) -> PIL images."""
-        probe = np.asarray(frames_style[0].convert("RGB") if isinstance(frames_style[0], Image.Image) else frames_style[0])
-        engine = PyramidPatchMatcher(image_height=probe.shape[0], image_width=probe.shape[1], channel=3, **ebsynth_config)
-        nv.require_cuda(engine.device, "FastBlend")
-        style = stage_frames(frames_style, engine.device)
-        guide = style if frames_guide is frames_style else stage_frames(frames_guide, engine.device)
-        if len(guide) != len(style) or guide[0].data.shape != style[0].data.shape:
-            raise ValueError("FastBlend: original and rendered frames must be as many and of one size")
-        tm = TableManager()
-        table_l = tm.build_remapping_table(guide, style, engine, batch_size)
-        table_l = tm.process_window_sum(guide, tm.remapping_table_to_blending_table(table_l), engine, window_size, batch_size)
-        table_r = tm.build_remapping_table(guide[::-1], style[::-1], engine, batch_size)
-        table_r = tm.process_window_sum(guide[::-1], tm.remapping_table_to_blending_table(table_r), engine, window_size,
-                                        batch_size)[::-1]
-        H, W = probe.shape[:2]
-        out = torch.empty(len(style), H, W, 3, dtype=torch.uint8, device=engine.device)
-        for i, ((fl, wl), fm, (fr, wr)) in enumerate(zip(table_l, style, table_r)):
-            w = wl - 1 + wr                                         # the reference's weight_m = -1
-            nv.fastblend_table(nv.FB_WSUM, out[i], fl.data, wl / w, fm.data, -1 / w, c=fr.data, sc=wr / w,
-                               a_u8=fl.kind == "uint8", b_u8=True, c_u8=fr.kind == "uint8")
-        return [Image.fromarray(f) for f in out.cpu().numpy()]
+        """Frames (PIL images or uint8 [H, W, 3] arrays) -> PIL images.  The fast mode keeps the reference's per-frame
+        target style and plain patch error, without tracking: those options raise ValueError here (the balanced and
+        accurate modes and keyframe interpolation, in `.runners`, are where they apply)."""
+        for option, why in (("use_mean_target_style", "the accurate mode's option (runners.AccurateModeRunner)"),
+                            ("use_pairwise_patch_error", "keyframe interpolation's option (runners.InterpolationModeRunner)"),
+                            ("tracking_window_size", "the fast mode does not track")):
+            if ebsynth_config.get(option):
+                raise _unsupported(option, ebsynth_config[option], why)
+        return fast_mode(frames_guide, frames_style, batch_size, window_size, ebsynth_config)
 
     def __call__(self, rendered_frames, original_frames=None, **kwargs):
         frames = self.run(rendered_frames if original_frames is None else original_frames, rendered_frames,
