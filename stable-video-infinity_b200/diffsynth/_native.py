@@ -2,7 +2,7 @@
 ``include/svi_b200_lora.h``, ``include/svi_b200_rife.h``, ``include/svi_b200_esrgan.h``,
 ``include/svi_b200_fastblend.h``, ``include/svi_b200_fastblend_modes.h``,
 ``include/svi_b200_unianimate.h``, ``include/svi_b200_replace.h``,
-``include/svi_b200_quality.h`` and ``include/svi_b200_reward.h``).
+``include/svi_b200_quality.h``, ``include/svi_b200_reward.h`` and ``include/svi_b200_processors.h``).
 
 This is the only door between the Python host code and the hand-written sm_90a kernels.  There is no
 fallback: if the shared library is missing or a call fails, a ``RuntimeError`` is raised.
@@ -284,6 +284,14 @@ REWARD_SIGNATURES = {
     "svi_reward_head": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _f32, _vp, _vp]),
 }
 
+# the same for include/svi_b200_processors.h
+PROCESSORS_SIGNATURES = {
+    "svi_luma_sum_u8": (_i32, [_vp, _i32, _i64, _vp, _vp]),
+    "svi_enhance_blend_u8": (_i32, [_vp, _i32, _i64, _vp, _f32, _vp, _vp]),
+    "svi_sharpen_u8": (_i32, [_vp, _i32, _i32, _i32, _f32, _vp, _vp]),
+    "svi_rife_average_u8": (_i32, [_vp, _vp, _i32, _i64, _vp, _vp]),
+}
+
 _lib = None
 
 
@@ -303,7 +311,7 @@ def load():
     lib = ctypes.CDLL(_LIB_PATH)
     for name, (res, args) in (SIGNATURES | LORA_SIGNATURES | RIFE_SIGNATURES | ESRGAN_SIGNATURES |
                         FASTBLEND_SIGNATURES | FASTBLEND_MODES_SIGNATURES | UNIANIMATE_SIGNATURES | REPLACE_SIGNATURES | QUALITY_SIGNATURES |
-                        REWARD_SIGNATURES).items():
+                        REWARD_SIGNATURES | PROCESSORS_SIGNATURES).items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing: fail loudly
         fn.restype = res
         fn.argtypes = args
@@ -1476,4 +1484,55 @@ def reward_head(x, n_seq, w, bias, out):
     _check(load().svi_reward_head(_ptr(x, torch.float32, "x"), ldx, n_seq, x.shape[0] // n_seq, x.shape[1],
                                   _ptr(w, torch.float32, "w"), float(bias), _ptr(out, torch.float32, "out"), _stream()),
            "svi_reward_head")
+    return out
+
+
+# --------------------------------------------------------------------------------------------- processors (include/svi_b200_processors.h)
+def _u8_frames(t, name):
+    """(F, H, W) of a contiguous uint8 [F, H, W, 3] CUDA tensor"""
+    if t.dtype != torch.uint8 or t.dim() != 4 or t.shape[3] != 3 or not t.is_contiguous():
+        raise RuntimeError(f"svi_b200: {name} must be contiguous uint8 [F, H, W, 3], got {t.dtype} {tuple(t.shape)}")
+    _ptr(t, torch.uint8, name)
+    return t.shape[:3]
+
+
+def luma_sum_u8(rgb, sums):
+    """sums int64 [F] = per frame, the integer sum of Pillow's L of uint8 rgb [F, H, W, 3] (svi_luma_sum_u8)."""
+    F, H, W = _u8_frames(rgb, "rgb")
+    if sums.dtype != torch.int64 or tuple(sums.shape) != (F,):
+        raise RuntimeError("svi_b200.luma_sum_u8: sums must be int64 [F]")
+    _check(load().svi_luma_sum_u8(_ptr(rgb), F, H * W, _contig(sums, torch.int64, "sums"), _stream()), "svi_luma_sum_u8")
+    return sums
+
+
+def enhance_blend_u8(rgb, degenerate, rate, out):
+    """out uint8 [F, H, W, 3] = Image.blend(degenerate[f], rgb[f], rate) per frame; degenerate f32 [F] (svi_enhance_blend_u8)."""
+    F, H, W = _u8_frames(rgb, "rgb")
+    if out.shape != rgb.shape or tuple(degenerate.shape) != (F,):
+        raise RuntimeError("svi_b200.enhance_blend_u8: out must have rgb's shape and degenerate one value per frame")
+    _u8_frames(out, "out")
+    _check(load().svi_enhance_blend_u8(_ptr(rgb), F, H * W, _contig(degenerate, torch.float32, "degenerate"), float(rate),
+                                       _ptr(out), _stream()), "svi_enhance_blend_u8")
+    return out
+
+
+def sharpen_u8(rgb, rate, out):
+    """out uint8 [F, H, W, 3] = Image.blend(rgb.filter(SMOOTH), rgb, rate) per frame (svi_sharpen_u8)."""
+    F, H, W = _u8_frames(rgb, "rgb")
+    if out.shape != rgb.shape:
+        raise RuntimeError("svi_b200.sharpen_u8: out must have rgb's shape")
+    _u8_frames(out, "out")
+    _check(load().svi_sharpen_u8(_ptr(rgb), F, H, W, float(rate), _ptr(out), _stream()), "svi_sharpen_u8")
+    return out
+
+
+def rife_average_u8(frames, merged, out):
+    """out[1:-1] uint8 RGB = ((frames[1:-1] + merged) / 2 * 255).clip(0, 255) truncated, from f32 BGR frames
+    [F, H, W, 4] and merged [F - 2, H, W, 4]; out [F, H, W, 3] keeps its first and last frames (svi_rife_average_u8)."""
+    F, H, W = _u8_frames(out, "out")
+    if tuple(frames.shape) != (F, H, W, 4) or tuple(merged.shape) != (F - 2, H, W, 4):
+        raise RuntimeError("svi_b200.rife_average_u8: frames must be [F, H, W, 4] and merged [F - 2, H, W, 4] for out "
+                           "[F, H, W, 3]")
+    _check(load().svi_rife_average_u8(_contig(frames, torch.float32, "frames"), _contig(merged, torch.float32, "merged"),
+                                      F, H * W, _ptr(out), _stream()), "svi_rife_average_u8")
     return out

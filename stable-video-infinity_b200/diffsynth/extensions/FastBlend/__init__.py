@@ -331,15 +331,22 @@ class TableManager:
 
 
 def stage_frames(frames, device):
-    """uint8 RGB frames (PIL images or [H, W, 3] arrays) -> `Frame`s on the device (one upload, one staging launch)."""
-    arrs = [np.asarray(f.convert("RGB") if isinstance(f, Image.Image) else f) for f in frames]
-    if not arrs:
-        raise ValueError("FastBlend: no frames")
-    H, W = arrs[0].shape[:2]
-    if any(a.dtype != np.uint8 or a.shape != (H, W, 3) for a in arrs):
-        raise ValueError("FastBlend: frames must be uint8 RGB of one size (PIL images or [H, W, 3] arrays)")
-    u8 = torch.from_numpy(np.stack(arrs)).to(device)
-    staged = nv.fastblend_stage_frames(u8, torch.empty(len(arrs), H, W, 4, dtype=torch.float32, device=device))
+    """uint8 RGB frames (PIL images or [H, W, 3] arrays, or one uint8 [F, H, W, 3] tensor, which stays on the device)
+    -> `Frame`s on the device (one upload, one staging launch)."""
+    if torch.is_tensor(frames):
+        if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3 or frames.shape[0] == 0:
+            raise ValueError("FastBlend: a frame tensor must be uint8 [F, H, W, 3]")
+        u8 = frames.to(device).contiguous()
+    else:
+        arrs = [np.asarray(f.convert("RGB") if isinstance(f, Image.Image) else f) for f in frames]
+        if not arrs:
+            raise ValueError("FastBlend: no frames")
+        H, W = arrs[0].shape[:2]
+        if any(a.dtype != np.uint8 or a.shape != (H, W, 3) for a in arrs):
+            raise ValueError("FastBlend: frames must be uint8 RGB of one size (PIL images or [H, W, 3] arrays)")
+        u8 = torch.from_numpy(np.stack(arrs)).to(device)
+    F, H, W, _ = u8.shape
+    staged = nv.fastblend_stage_frames(u8, torch.empty(F, H, W, 4, dtype=torch.float32, device=device))
     return [Frame(f, "uint8") for f in staged]
 
 
@@ -354,13 +361,15 @@ def stage_pair(frames_guide, frames_style, device):
 
 
 def frame_size(frame):
-    """(H, W) of a PIL image or [H, W, 3] array"""
+    """(H, W) of a PIL image or [H, W, 3] array or tensor"""
+    if torch.is_tensor(frame):
+        return tuple(frame.shape[:2])
     return np.asarray(frame.convert("RGB") if isinstance(frame, Image.Image) else frame).shape[:2]
 
 
 def fast_mode(frames_guide, frames_style, batch_size, window_size, ebsynth_config):
     """The fast mode (runners/fast.py, __init__.py): the left and right tree tables and their merge.  Frames (PIL images
-    or uint8 [H, W, 3] arrays) -> PIL images."""
+    or uint8 [H, W, 3] arrays) -> PIL images; frames_style as a uint8 [F, H, W, 3] tensor -> a tensor on the device."""
     H, W = frame_size(frames_style[0])
     engine = PyramidPatchMatcher(image_height=H, image_width=W, channel=3, **ebsynth_config)
     nv.require_cuda(engine.device, "FastBlend")
@@ -376,6 +385,8 @@ def fast_mode(frames_guide, frames_style, batch_size, window_size, ebsynth_confi
         w = wl - 1 + wr                                         # the reference's weight_m = -1
         nv.fastblend_table(nv.FB_WSUM, out[i], fl.data, wl / w, fm.data, -1 / w, c=fr.data, sc=wr / w,
                            a_u8=fl.kind == "uint8", b_u8=True, c_u8=fr.kind == "uint8")
+    if torch.is_tensor(frames_style):
+        return out
     return [Image.fromarray(f) for f in out.cpu().numpy()]
 
 

@@ -4,7 +4,8 @@ deflicker modes and keyframe interpolation, on the native kernels.
 Each runner keeps the reference's signature, task order and batching (the batch composition changes the bits: see
 PyramidPatchMatcher), writes `%05d.png` into `save_path` when one is given, and returns the frames as PIL images in
 frame order (the reference returns None).  Frames go in as PIL images or uint8 [H, W, 3] arrays and cross the bus once
-as bytes in each direction; everything between stays on the device.
+as bytes in each direction; everything between stays on the device.  The fast, balanced and accurate runners also take
+the frames as a uint8 [F, H, W, 3] tensor, and then return the output as a uint8 tensor on the device.
 
 Kept from the reference on purpose:
   - Balanced saves each frame's blend as it stood *before* its last neighbour was added (runners/balanced.py clips the
@@ -24,7 +25,9 @@ from . import Frame, PyramidPatchMatcher, fast_mode, frame_size, stage_frames, s
 
 
 def _raw(frames):
-    """the reference's VideoData (`raw_data()`) or a sequence of frames -> a list of frames"""
+    """the reference's VideoData (`raw_data()`) or a sequence of frames -> a list of frames; a frame tensor as it is"""
+    if torch.is_tensor(frames):
+        return frames
     return frames.raw_data() if hasattr(frames, "raw_data") else list(frames)
 
 
@@ -32,13 +35,16 @@ def _stack(frames):
     return torch.stack([f.data for f in frames])
 
 
-def _finish(out, save_path):
-    """uint8 [n, H, W, 3] on the device -> PIL images, saved as %05d.png when save_path is given"""
+def _finish(out, save_path, frames_style=None):
+    """uint8 [n, H, W, 3] on the device -> PIL images (or `out` itself when frames_style is a tensor), saved as
+    %05d.png when save_path is given"""
+    if save_path is None and torch.is_tensor(frames_style):
+        return out
     images = [Image.fromarray(f) for f in out.cpu().numpy()]
     if save_path is not None:
         for i, image in enumerate(images):
             image.save(os.path.join(save_path, "%05d.png" % i))
-    return images
+    return out if torch.is_tensor(frames_style) else images
 
 
 def _engine(frames_style, ebsynth_config, **options):
@@ -54,7 +60,7 @@ class FastModeRunner:
     def run(self, frames_guide, frames_style, batch_size, window_size, ebsynth_config, save_path=None):
         frames = fast_mode(_raw(frames_guide), _raw(frames_style), batch_size, window_size, ebsynth_config)
         if save_path is not None:
-            for i, image in enumerate(frames):
+            for i, image in enumerate(frames if not torch.is_tensor(frames) else _finish(frames, None)):
                 image.save(os.path.join(save_path, "%05d.png" % i))
         return frames
 
@@ -90,7 +96,7 @@ class BalancedModeRunner:
                 if weight + 1 == min(n, target + window_size + 1) - max(0, target - window_size):
                     nv.fastblend_to_u8(frame.data, out[target], a_u8=frame.kind == "uint8")   # the blend before this one
                     frames[target] = (None, 1)
-        return _finish(out, save_path)
+        return _finish(out, save_path, frames_style)
 
 
 class AccurateModeRunner:
@@ -117,7 +123,7 @@ class AccurateModeRunner:
                 remapped.append(ts)
             nv.fastblend_batch_mean(torch.cat(remapped), mean)
             nv.fastblend_to_u8(mean, out[target])
-        return _finish(out, save_path)
+        return _finish(out, save_path, frames_style)
 
 
 def _check_keyframes(index_style, frames_style, n, single):
